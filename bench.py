@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - throughput of librsem_b200's EM / Gibbs hot path on B200, and the reference's CPU arm.
+"""bench.py - throughput of librsem_b200's EM / Gibbs hot path on H100, and the reference's CPU arm.
 
 Metric (BASELINE.json): EM reads*hits/s (= hits streamed per second by the frozen-conprb E+M round, rounds >= 12 of the
 reference's EM loop) and the equivalent EM iterations/s; HBM GB/s against the roofline.
@@ -13,7 +13,7 @@ reference's EM loop) and the equivalent EM iterations/s; HBM GB/s against the ro
   python bench.py --impl reference                       # oracle/_ref/rsem-run-em (the unmodified reference) on the host cores
 
 A "step" is one EM round = K2 (E-step + count accumulation) [+ NCCL allreduce of the count vector when N > 1] + K4 (theta
-update, convergence test) over the resident hit matrix.  The matrix (>= 9 GB at C3) is far larger than L2 (126 MB), so
+update, convergence test) over the resident hit matrix.  The matrix (>= 9 GB at C3) is far larger than L2 (50 MB), so
 no explicit L2 flush is needed; C1 fits L2 and says so.
 """
 from __future__ import annotations
@@ -118,7 +118,7 @@ def small_matrix_numpy(N, M, deg, seed):
 
 
 class ClockSampler:
-    """nvidia-smi sampling while the GPU runs the timed workload (B200_PROFILING.md 'clocks' recipe).
+    """nvidia-smi sampling while the GPU runs the timed workload.
     nvidia-smi needs ~0.2 s to start and samples every 100 ms, so it is started before the warm-up and only
     samples whose time stamp lies inside [t0, t1] (GPU under the benchmark's load) are used."""
     Q = ("timestamp,index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -188,7 +188,19 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(d, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array (float64), so that two builds can be compared output for output"""
+    total = sum(np.asarray(a).nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, f"outputs of {total} bytes exceed the {DUMP_LIMIT} byte dump limit"
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def git_head():
@@ -410,6 +422,8 @@ def run_ours(args):
         e1.record(stream)
     barrier()
     launches = ctx.launch_count() - l0
+    if args.dump_outputs and rank == 0:  # what the last timed round handed back, before any further round runs
+        dump_outputs(args.dump_outputs, {"theta": ctx.get_theta(), "round_stats": np.array(stats[-1], np.float64)})
     cta_ns = ctx.estep_cta_times().astype(np.float64)
     # keep the same load running until nvidia-smi has a few samples of it (a 20-round region lasts 50 ms)
     extra = 0
@@ -506,7 +520,7 @@ def run_ours(args):
                 dist.all_reduce(t, op=dist.ReduceOp.MAX)
                 times = [float(x) for x in t.tolist()]
             assert abs(th.sum() - 1.0) < 1e-9
-            dt = sorted(times)[len(times) // 2]   # median job: about one upload_hits in four takes 3-5x longer (cause not identified), see profiles/README.md
+            dt = sorted(times)[len(times) // 2]   # median job: an occasional upload_hits takes several times longer
             res[rounds] = (total_hits * rounds / dt, dt, [round(x, 4) for x in times])
         r0 = E2E_ROUNDS[0]
         e2e = {"value": res[r0][0], "unit": "hits/s", "h2d_bytes_per_step": bytes_in // r0, "d2h_bytes_per_step": bytes_out // r0,
@@ -696,7 +710,11 @@ def main():
     ap.add_argument("--gibbs-reads", type=int, default=10_000_000)
     ap.add_argument("--gibbs-chains", type=int, default=8)
     ap.add_argument("--model-reads", type=int, default=2_000_000)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed round returned (theta, its round statistics) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload not in WORKLOADS):
+        ap.error("--dump-outputs applies to the EM workloads of --impl ours")
     args.warmup = max(args.warmup, 3)
     # pin the OpenMP threads of the cpu_baseline leg before any OpenMP runtime starts
     os.environ.setdefault("OMP_PROC_BIND", "spread")

@@ -1,5 +1,5 @@
 /*
- * rsem_b200.h - C ABI of librsem_b200.so: the B200 (sm_100a) implementation of RSEM's
+ * rsem_b200.h - C ABI of librsem_b200.so: the H100 (sm_90a) implementation of RSEM's
  * expression-estimation hot path (rsem-run-em E/M loop and rsem-run-gibbs sampler).
  *
  * The reference has no in-process plugin/FFI interface for this path: its boundary is the

@@ -1,4 +1,4 @@
-"""rsem_b200 - B200 (sm_100a) implementation of RSEM's EM / Gibbs estimation hot path.
+"""rsem_b200 - H100 (sm_90a) implementation of RSEM's EM / Gibbs estimation hot path.
 
 The product is `librsem_b200.so` (hand-written CUDA behind the C ABI of include/rsem_b200.h) and the
 drop-in executables `bin/rsem-run-em` / `bin/rsem-run-gibbs` (C++ hosts in rsem_b200/host/).  This

@@ -1,6 +1,6 @@
 """In-tree build of every native artefact (called by __graft_entry__.build()).
 
-  rsem_b200/librsem_b200.so   CUDA kernels + C ABI, sm_100a only
+  rsem_b200/librsem_b200.so   CUDA kernels + C ABI, sm_90a only
   bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments   C++ drop-in executables (link the .so)
   tools/gen_dataset           synthetic intermediate-file generator (tooling)
   oracle/librsem_oracle.so    CPU restatement (test infrastructure)
@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "rsem_b200", "csrc")
 HOST = os.path.join(ROOT, "rsem_b200", "host")
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "-diag-suppress", "177"]
 
 
@@ -64,11 +64,11 @@ def build_tools(force: bool = False):
     out = os.path.join(ROOT, "tools", "gen_dataset")
     if force or _newer(out, [src]):
         _run(["g++", "-O2", "-std=c++17", "-o", out, src])
-    # micro-benchmark behind the lane-mapping table in profiles/README.md (tools/gpu/red_bench.sh)
+    # micro-benchmark: red / ldg throughput per lane mapping
     src = os.path.join(ROOT, "tools", "micro", "red_bench.cu")
     out = os.path.join(ROOT, "tools", "micro", "red_bench")
     if os.path.exists(src) and (force or _newer(out, [src])):
-        _run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-o", out, src])
+        _run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-o", out, src])
 
 
 def build_oracle():

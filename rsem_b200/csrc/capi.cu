@@ -243,9 +243,9 @@ int rsem_b200_ctx_create(int device, rsem_b200_ctx** out) {
     RB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     RB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {
         char buf[256];
-        snprintf(buf, sizeof buf, "device %d is sm_%d%d; librsem_b200 contains sm_100a code only", device, prop.major,
+        snprintf(buf, sizeof buf, "device %d is sm_%d%d; librsem_b200 contains sm_90a code only", device, prop.major,
                  prop.minor);
         set_error(buf);
         return RSEM_B200_ERR_UNSUPPORTED;

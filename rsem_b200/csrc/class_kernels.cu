@@ -991,7 +991,7 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         unsigned grid = (unsigned)ctx->sm_count;
         if (grid > L.n_tiles) grid = L.n_tiles;
         L.last_grid = grid;
-        // consumer warps x rows in flight per lane; measured on C3 in profiles/README.md
+        // consumer warps x rows in flight per lane
         switch (L.threads) {
 #define RB_CLASS_LAUNCH(W, U)                                                                                   \
     {                                                                                                           \

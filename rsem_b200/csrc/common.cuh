@@ -150,7 +150,7 @@ struct ClassLayout {
 
 struct rsem_b200_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;   // host -> device copies that overlap with work on `stream` (upload_conprb)

@@ -3,7 +3,7 @@
 //
 // What they compute is the reference's E_STEP inner loops (/root/reference/EM.cpp:199-244) and
 // the M-step + relative-change statistics (/root/reference/EM.cpp:385-416).  How they compute
-// it is specific to sm_100a:
+// it is specific to sm_90a:
 //
 //   * the hit matrix is SoA CSR in HBM (row_ptr u64, sid i32, conprb f64, ncpv f64); one pass
 //     streams 12 B per hit + 16 B per read, nothing else comes from HBM (theta / count live in L2);

@@ -10,7 +10,7 @@
 //                    PairedEndQModel.h:161-188  (+ Profile.h:91-96, QProfile.h:88-93,
 //                    NoiseProfile.h:71-76, NoiseQProfile.h:74-79, LenDist.h:46-49, RSPD.h:43-59)
 //
-// B200 mapping: reads (base codes + qualities) and transcripts are resident in HBM, parsed once
+// H100 mapping: reads (base codes + qualities) and transcripts are resident in HBM, parsed once
 // (the reference re-parses the FASTA/FASTQ text every round).  A read is handled by a group of G
 // lanes (the same grouping as the E-step); each lane walks the bases of its own hits.  The
 // (Q)Profile table is staged in shared memory.  K3 accumulates with red.global.add.f64 into

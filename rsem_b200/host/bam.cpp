@@ -286,7 +286,7 @@ AlnReader::AlnReader(const std::string& path) : src_(new Source) {
     uint8_t magic[4] = {0, 0, 0, 0};
     const size_t got = fread(magic, 1, 4, probe);
     fclose(probe);
-    if (got >= 4 && !memcmp(magic, "CRAM", 4)) die("rsem-run-em (B200): CRAM input for -b is not supported; convert it to BAM (convert-sam-for-rsem).");
+    if (got >= 4 && !memcmp(magic, "CRAM", 4)) die("rsem-run-em (H100): CRAM input for -b is not supported; convert it to BAM (convert-sam-for-rsem).");
     uint8_t head[18] = {0};
     {
         FILE* p2 = fopen(path.c_str(), "rb");

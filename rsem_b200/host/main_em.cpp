@@ -1,4 +1,4 @@
-// rsem-run-em, B200 edition: same argv, same input and output files as the reference executable
+// rsem-run-em, H100 edition: same argv, same input and output files as the reference executable
 // (/root/reference/EM.cpp:541-675), so it drops in beside the unmodified rsem-calculate-expression.
 //
 //   rsem-run-em refName read_type sampleName imdName statName [-p #Threads] [-b samInpF has_fai? [fai_file]]

@@ -1,4 +1,4 @@
-// rsem-run-gibbs, B200 edition: same argv and files as the reference (/root/reference/Gibbs.cpp:425-530).
+// rsem-run-gibbs, H100 edition: same argv and files as the reference (the reference's Gibbs.cpp:425-530).
 //
 //   rsem-run-gibbs reference_name imdName statName BURNIN NSAMPLES GAP [-p #Threads] [--seed seed]
 //                  [--pseudo-count pseudo_count] [--prior file] [-q]

@@ -1,4 +1,4 @@
-// rsem-parse-alignments, B200 edition: the caller-side hand-off of the hot path (SURVEY.md 8(f).2).
+// rsem-parse-alignments, H100 edition: the caller-side hand-off of the hot path (SURVEY.md 8(f).2).
 //
 //   rsem-parse-alignments refName imdName statName alignF read_type [-t fai_file] [-tag tagName] [-q]
 //
@@ -310,7 +310,7 @@ int main(int argc, char* argv[]) {
     Parser ps;
     for (int i = 6; i < argc; ++i) {
         if (!strcmp(argv[i], "-t") && i + 1 < argc)
-            fprintf(stderr, "Warning: rsem-parse-alignments (B200): -t %s is ignored (a FASTA index is only needed for CRAM, which is not supported).\n", argv[i + 1]);
+            fprintf(stderr, "Warning: rsem-parse-alignments (H100): -t %s is ignored (a FASTA index is only needed for CRAM, which is not supported).\n", argv[i + 1]);
         if (!strcmp(argv[i], "-tag") && i + 1 < argc) ps.rt_tag = argv[i + 1];
         if (!strcmp(argv[i], "-q")) g_verbose = false;
     }

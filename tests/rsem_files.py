@@ -1,8 +1,13 @@
 """Readers for RSEM's intermediate / output files, and helpers that run the reference binaries
 (oracle/_ref) and the drop-in executables (bin/) on a generated dataset.  Test infrastructure."""
+import hashlib
+import io
+import json
 import os
 import shutil
 import subprocess
+import tarfile
+import types
 
 import numpy as np
 
@@ -10,10 +15,73 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 BIN_DIR = os.path.join(ROOT, "bin")
 GEN = os.path.join(ROOT, "tools", "gen_dataset")
+REF_RUNS = os.path.join(ROOT, "tests", "golden", "reference")
+# not stored: read indices are rebuilt from the reads; .ofg and BAM files of even the small cases are hundreds of KB
+UNSTORED = (".ridx", ".ofg", ".bam")
 
 
 def have_ref():
     return all(os.path.exists(os.path.join(REF_DIR, b)) for b in ("rsem-run-em-rounds", "rsem-run-gibbs", "rsem-build-read-index"))
+
+
+def _tree_digests(d):
+    out = {}
+    for dp, _, fs in os.walk(d):
+        for f in fs:
+            p = os.path.join(dp, f)
+            with open(p, "rb") as fh:
+                out[os.path.relpath(p, d)] = hashlib.sha256(fh.read()).hexdigest()
+    return out
+
+
+def _add_bytes(tar, name, data):
+    ti = tarfile.TarInfo(name)
+    ti.size = len(data)
+    tar.addfile(ti, io.BytesIO(data))
+
+
+def reference_run(key, d, run, out=None, digests_only=False):
+    """What a reference binary prints and writes when run on the data set in directory d (into d, or into out).
+
+    With oracle/_ref present, run() executes it (and RSEM_B200_RECORD_REFERENCE=1 stores the result as
+    tests/golden/reference/<key>.tar.xz: stdout, stderr, the files the run created or changed apart from UNSTORED,
+    and a digest of the input files).  Without it, those outputs are restored from the stored copy, after checking
+    that d holds the same inputs the reference was run on.  digests_only: for outputs that are compared byte for byte,
+    only the SHA-256 of each file is stored; the result's .digests maps each file the run wrote to its digest."""
+    out = out or d
+    inputs = hashlib.sha256(repr(sorted(_tree_digests(d).items())).encode()).hexdigest()
+    before = _tree_digests(out)
+    path = os.path.join(REF_RUNS, key + ".tar.xz")
+    if have_ref():
+        p = run()
+        p.digests = {rel: h for rel, h in _tree_digests(out).items() if before.get(rel) != h and not rel.endswith(UNSTORED)}
+        if os.environ.get("RSEM_B200_RECORD_REFERENCE") == "1":
+            os.makedirs(REF_RUNS, exist_ok=True)
+            with tarfile.open(path, "w:xz") as tar:
+                for name, text in (("inputs.sha256", inputs), ("returncode", str(p.returncode)), ("stdout", p.stdout or ""),
+                                   ("stderr", p.stderr or "")):
+                    _add_bytes(tar, name, text.encode())
+                if digests_only:
+                    _add_bytes(tar, "digests.json", json.dumps(p.digests, sort_keys=True).encode())
+                else:
+                    for rel in sorted(p.digests):
+                        tar.add(os.path.join(out, rel), arcname="files/" + rel)
+        return p
+    if not os.path.exists(path):
+        import pytest
+        pytest.skip(f"needs oracle/_ref or tests/golden/reference/{key}.tar.xz")
+    with tarfile.open(path) as tar:
+        text = {n: tar.extractfile(n).read().decode() for n in ("inputs.sha256", "returncode", "stdout", "stderr")}
+        assert text["inputs.sha256"] == inputs, f"{key}: the generated inputs differ from those the reference was run on"
+        names = tar.getnames()
+        digests = json.loads(tar.extractfile("digests.json").read()) if "digests.json" in names else None
+        for m in tar.getmembers():
+            if m.name.startswith("files/"):
+                m.name = m.name[len("files/"):]
+                tar.extract(m, out, filter="data")
+    if digests is None:
+        digests = {rel: h for rel, h in _tree_digests(out).items() if before.get(rel) != h}
+    return types.SimpleNamespace(returncode=int(text["returncode"]), stdout=text["stdout"], stderr=text["stderr"], digests=digests)
 
 
 def gen_dataset(out, **kw):

@@ -29,7 +29,7 @@ def test_library_exports_every_declared_symbol(built):
     assert rsem_b200.load_library().version() == 100
 
 
-def test_no_cpu_fallback(built):
+def test_no_cpu_fallback(built, tmp_path):
     """without a CUDA device every path fails loudly: the library returns an error, the executables exit(-1)"""
     import torch
     if torch.cuda.is_available():
@@ -37,7 +37,7 @@ def test_no_cpu_fallback(built):
     import rsem_b200
     with pytest.raises(rsem_b200.RsemB200Error):
         rsem_b200.Context(0)
-    d = rf.gen_dataset("/tmp/rsem_b200_nogpu_case", read_type=0, M=20, N1=50, N0=5)
+    d = rf.gen_dataset(str(tmp_path / "d"), read_type=0, M=20, N1=50, N0=5)
     p = rf.run_em(d, 0, "ours", rounds=2, check=False)
     assert p.returncode == 255 and "CUDA" in p.stderr
 

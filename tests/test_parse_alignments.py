@@ -3,7 +3,8 @@
 Reference behaviour: /root/reference/parseIt.cpp:64-229, SamParser.h:97-265, Transcripts.h:105-143.
   * every output file (.dat, the read files per category, .cnt, .omit) is BYTE-IDENTICAL to what the reference's
     rsem-parse-alignments (oracle/_ref, built from the reference sources with its vendored htslib) writes, for all four
-    read types, SAM and BAM input, and with the aligner's "too many alignments" tag (-tag, the N2 category);
+    read types, SAM and BAM input, and with the aligner's "too many alignments" tag (-tag, the N2 category); without
+    oracle/_ref, compared by SHA-256 with the digests stored from it (tests/golden/reference);
   * imd.b200 holds the same hits and reads as the text files: compared array by array with what the text parsers of
     rsem-run-em produce from the files next to it (rsem-b200-host-selftest dumps both), including the low-quality flags
     and the names of the reads shorter than the seed length; a stale side-car (text file replaced) is refused.
@@ -22,7 +23,6 @@ OURS = os.path.join(ROOT, "bin", "rsem-parse-alignments")
 REF = os.path.join(rf.REF_DIR, "rsem-parse-alignments")
 SELFTEST = os.path.join(ROOT, "bin", "rsem-b200-host-selftest")
 
-needs_ref = pytest.mark.skipif(not os.path.exists(REF), reason="needs oracle/_ref/rsem-parse-alignments (oracle/Makefile)")
 
 
 def _parse(exe, d, aln, read_type, out, extra=()):
@@ -44,25 +44,37 @@ def _assert_same_tree(a, b):
         assert filecmp.cmp(os.path.join(a, f), os.path.join(b, f), shallow=False), f"{f} differs"
 
 
-@needs_ref
+def _ref_parse(key, d, aln, read_type, out, extra=()):
+    """the reference's rsem-parse-alignments on d, or the digests of what it wrote (rsem_files.reference_run)"""
+    return rf.reference_run(key, d, lambda: _parse(REF, d, aln, read_type, out, extra), out=out, digests_only=True)
+
+
+def _assert_same_as_reference(r, ours):
+    """every file the reference wrote, byte for byte (by SHA-256), and no other"""
+    mine = {f: h for f, h in rf._tree_digests(ours).items() if not f.endswith(".b200")}
+    assert sorted(mine) == sorted(r.digests), (sorted(mine), sorted(r.digests))
+    for f, h in r.digests.items():
+        assert mine[f] == h, f"{f} differs"
+
+
 @pytest.mark.parametrize("read_type", [0, 1, 2, 3])
 def test_outputs_byte_identical_to_the_reference(built, tmp_path, read_type):
     d = rf.gen_dataset(str(tmp_path / "d"), read_type=read_type, M=150, N1=3000, N0=200, read_len=50, var_len=30, seed=5 + read_type,
                        sam=1, spurious=0.05, omit=7)
     sam = f"{d}/aln.sam"
-    r = _parse(REF, d, sam, read_type, str(tmp_path / "ref"))
+    r = _ref_parse(f"parse_{read_type}", d, sam, read_type, str(tmp_path / "ref"))
     o = _parse(OURS, d, sam, read_type, str(tmp_path / "ours"))
     assert r.returncode == 0 and o.returncode == 0, (r.stderr, o.stderr)
-    _assert_same_tree(str(tmp_path / "ref"), str(tmp_path / "ours"))
+    _assert_same_as_reference(r, str(tmp_path / "ours"))
     assert os.path.getsize(tmp_path / "ours" / "t" / "s.dat") > 1000
     # the reference's .dat equals the generator's hand-written one up to the padded header line (SURVEY 8(c))
     # BAM input (converted by this repository's own BGZF writer): same files again, from both programs
-    bam = str(tmp_path / "aln.bam")
+    bam = f"{d}/aln.bam"
     subprocess.check_call([SELFTEST, "--bam-copy", sam, bam, "2"], stdout=subprocess.DEVNULL)
-    rb = _parse(REF, d, bam, read_type, str(tmp_path / "ref_bam"))
+    rb = _ref_parse(f"parse_{read_type}_bam", d, bam, read_type, str(tmp_path / "ref_bam"))
     ob = _parse(OURS, d, bam, read_type, str(tmp_path / "ours_bam"))
     assert rb.returncode == 0 and ob.returncode == 0, (rb.stderr, ob.stderr)
-    _assert_same_tree(str(tmp_path / "ref_bam"), str(tmp_path / "ours_bam"))
+    _assert_same_as_reference(rb, str(tmp_path / "ours_bam"))
     for f in _files(str(tmp_path / "ours")):
         if f.endswith(".dat") or f.endswith(".cnt") or ".f" in f:   # .omit differs only if the header differs: it does not
             assert filecmp.cmp(tmp_path / "ours" / f, tmp_path / "ours_bam" / f, shallow=False), f
@@ -92,15 +104,14 @@ def _tag_some_unaligned(sam_in, sam_out, paired):
     return sam_out
 
 
-@needs_ref
 @pytest.mark.parametrize("read_type", [1, 2])
 def test_too_many_alignments_tag(built, tmp_path, read_type):
     d = rf.gen_dataset(str(tmp_path / "d"), read_type=read_type, M=80, N1=1500, N0=400, read_len=40, seed=3, sam=1)
-    sam = _tag_some_unaligned(f"{d}/aln.sam", str(tmp_path / "tagged.sam"), read_type >= 2)
-    r = _parse(REF, d, sam, read_type, str(tmp_path / "ref"), ("-tag", "XM"))
+    sam = _tag_some_unaligned(f"{d}/aln.sam", f"{d}/tagged.sam", read_type >= 2)
+    r = _ref_parse(f"parse_tag_{read_type}", d, sam, read_type, str(tmp_path / "ref"), ("-tag", "XM"))
     o = _parse(OURS, d, sam, read_type, str(tmp_path / "ours"), ("-tag", "XM"))
     assert r.returncode == 0 and o.returncode == 0, (r.stderr, o.stderr)
-    _assert_same_tree(str(tmp_path / "ref"), str(tmp_path / "ours"))
+    _assert_same_as_reference(r, str(tmp_path / "ours"))
     n0, n1, n2, tot = (int(x) for x in open(tmp_path / "ours" / "s" / "s.cnt").readline().split())
     assert n2 > 50 and n0 > 50 and n0 + n1 + n2 == tot
     assert any(f.startswith("t/s_max") for f in _files(str(tmp_path / "ours")))

@@ -28,10 +28,8 @@ def slice_csr(row_ptr, first, last):
 
 @pytest.mark.parametrize("threads", [2, 3, 7])
 def test_shards_equal_reference_thread_split(tmp_path, built, threads):
-    if not rf.have_ref():
-        pytest.skip("oracle/_ref binaries not available")
     d = rf.gen_dataset(str(tmp_path / "d"), read_type=0, M=80, N1=900, N0=40, read_len=40, maxL=100, seed=threads)
-    p = rf.run_em(d, 0, "ref", rounds=1, min_rounds=1, threads=threads, gibbs_out=False)
+    p = rf.reference_run(f"shards_{threads}", d, lambda: rf.run_em(d, 0, "ref", rounds=1, min_rounds=1, threads=threads, gibbs_out=False))
     ref = [(int(a), int(b)) for a, b in re.findall(r"Thread \d+ : N = (\d+), NHit = (\d+)", p.stdout)]
     row_ptr, _, _, _ = rf.read_dat(f"{d}/s.temp/s.dat", False)
     mine = [(b - a, int(row_ptr[b] - row_ptr[a])) for a, b in shard_reads(row_ptr, threads)]

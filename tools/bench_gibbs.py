@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Whole-executable timing of rsem-run-gibbs (B200) against the reference on one generated dataset; checks that the
+"""Whole-executable timing of rsem-run-gibbs (H100) against the reference on one generated dataset; checks that the
 count vectors are byte-identical.  Tooling for profiles/."""
 import argparse
 import filecmp

@@ -4,7 +4,7 @@
 The reference ships no golden vectors for the EM / Gibbs path (SURVEY.md section 4), so parity is pinned against
 outputs of the reference itself: oracle/_ref/* are compiled by oracle/Makefile from the sources where they lie in
 /root/reference.  This script only runs in the build container (it needs oracle/_ref); the fixtures it writes are
-committed and are all the GPU box needs.
+committed and are all the tests need.
 
     python tools/make_golden.py            # regenerates every case (deterministic: fixed generator seeds)
 """

@@ -4,7 +4,7 @@
 //   mapping 1: pairs     entry = 64 * (i / 2) + 2 * lane + (i & 1)
 //   mapping 2: blocked4  entry = 4 * lane + i
 //   mapping 3: random    every lane its own random address (no locality at all)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o red_bench red_bench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o red_bench red_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
