@@ -243,6 +243,11 @@ int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 8 */);
 /* Busy time (ns, %globaltimer) of every persistent CTA in the latest class-layout E-step launch: the evidence for
  * the segmented reduction's load balance on skewed matrices (BASELINE configs[4]).  *n = CTAs written (<= cap).   */
 int rsem_b200_estep_cta_times(rsem_b200_ctx* ctx, uint64_t* out_ns, int32_t cap, int32_t* n);
+/* Where the class-layout E-step's time went in its latest launch with profiling on (rsem_b200_set_profiling):
+ * out_ns[3 i .. 3 i + 2] = { ns the consumer warps of CTA i spent blocked on staged data (summed over the warps),
+ * ns a separate copy-issuing warp spent blocked on a free stage (0 when the consumer warps issue their own copies),
+ * consumer warps of CTA i }.  *n = CTAs written (<= cap); 0 when the latest launch ran without profiling.          */
+int rsem_b200_estep_wait_times(rsem_b200_ctx* ctx, uint64_t* out_ns, int32_t cap, int32_t* n);
 
 #ifdef __cplusplus
 }

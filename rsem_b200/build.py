@@ -64,11 +64,12 @@ def build_tools(force: bool = False):
     out = os.path.join(ROOT, "tools", "gen_dataset")
     if force or _newer(out, [src]):
         _run(["g++", "-O2", "-std=c++17", "-o", out, src])
-    # micro-benchmark: red / ldg throughput per lane mapping
-    src = os.path.join(ROOT, "tools", "micro", "red_bench.cu")
-    out = os.path.join(ROOT, "tools", "micro", "red_bench")
-    if os.path.exists(src) and (force or _newer(out, [src])):
-        _run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-o", out, src])
+    # micro-benchmarks: red / ldg throughput per lane mapping; HBM read rate per copy geometry
+    for name in ("red_bench", "hbm_read"):
+        src = os.path.join(ROOT, "tools", "micro", name + ".cu")
+        out = os.path.join(ROOT, "tools", "micro", name)
+        if os.path.exists(src) and (force or _newer(out, [src])):
+            _run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-o", out, src])
 
 
 def build_oracle():

@@ -77,7 +77,7 @@ SYMBOLS = [
     "rsem_b200_em_rounds", "rsem_b200_em_model_round", "rsem_b200_expected_weights", "rsem_b200_gibbs_upload",
     "rsem_b200_gibbs_run", "rsem_b200_launch_count", "rsem_b200_estep_timing", "rsem_b200_set_profiling",
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
-    "rsem_b200_estep_cta_times",
+    "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times",
 ]
 
 
@@ -294,6 +294,14 @@ class Context:
         out = np.zeros(1024, np.uint64)
         n = C.c_int32(0)
         self.lib.check(self.lib.dll.rsem_b200_estep_cta_times(self._h, _p(out, C.c_uint64), C.c_int32(1024), C.byref(n)))
+        return out[: n.value]
+
+    def estep_wait_times(self) -> np.ndarray:
+        """per CTA of the latest profiled class-kernel launch: (consumer ns blocked on data summed over its warps,
+        copy-issuer ns blocked on a free stage, consumer warps); empty when that launch ran without profiling"""
+        out = np.zeros((1024, 3), np.uint64)
+        n = C.c_int32(0)
+        self.lib.check(self.lib.dll.rsem_b200_estep_wait_times(self._h, _p(out, C.c_uint64), C.c_int32(1024), C.byref(n)))
         return out[: n.value]
 
     def set_estep_variant(self, v: int):

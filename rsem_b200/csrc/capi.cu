@@ -770,6 +770,19 @@ int rsem_b200_estep_cta_times(rsem_b200_ctx* c, uint64_t* out_ns, int32_t cap, i
     return 0;
 }
 
+int rsem_b200_estep_wait_times(rsem_b200_ctx* c, uint64_t* out_ns, int32_t cap, int32_t* n) {
+    RB_ARG(c && out_ns && n, "NULL argument");
+    *n = 0;
+    const ClassLayout& L = c->cls;
+    if (!L.wait_ns || !L.last_profiled || L.last_grid == 0) return 0;
+    RB_CUDA(cudaSetDevice(c->device));
+    const int k = std::min<int>(cap, (int)L.last_grid);
+    RB_CUDA(cudaMemcpyAsync(out_ns, L.wait_ns, (size_t)k * 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    *n = k;
+    return 0;
+}
+
 int rsem_b200_set_estep_variant(rsem_b200_ctx* c, int32_t v) {
     RB_ARG(c && v >= 0 && v <= 5, "variant must be 0..5");
     c->variant = v;

@@ -91,6 +91,21 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
         "r"(parity)
         : "memory");
 }
+__device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+    return t;
+}
+// mbar_wait that adds the time it blocked to *acc when profiling (acc != nullptr); no timer read otherwise
+__device__ __forceinline__ void mbar_wait_timed(unsigned long long* bar, unsigned parity, unsigned long long* acc) {
+    if (acc) {
+        const unsigned long long t0 = global_ns();
+        mbar_wait(bar, parity);
+        *acc += global_ns() - t0;
+    } else {
+        mbar_wait(bar, parity);
+    }
+}
 __device__ __forceinline__ void bulk_load(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                      smem_u32(dst)),
@@ -348,6 +363,8 @@ struct ClassArgs {
     double* count;
     const int* done_flag;
     unsigned long long* cta_ns;  // per-CTA busy time of this launch (globaltimer, ns): load-balance evidence
+    unsigned long long* wait_ns;  // profiling only (else nullptr): per CTA {consumer ns blocked on data, producer ns
+                                  // blocked on a free stage, consumer warps}
 };
 
 struct StageDesc {  // written by the producer when it issues a tile
@@ -365,15 +382,16 @@ struct ClassSmem {
     unsigned long long empty_bar[kStages];  // consumers -> producer: every consumer warp is done with the stage
     StageDesc sd[kStages];
     double red[W + 1];
+    unsigned long long wait[2];
 };
 
 __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-__device__ __forceinline__ void issue_class_tile(const ClassArgs& a, unsigned k, unsigned char* st, unsigned long long* bar,
-                                                 StageDesc& sd, unsigned n_consumers) {
-    const TileRec t0 = a.tile[k], t1 = a.tile[k + 1];
+// t0, t1: the tile's records, loaded by the caller before it waits for the stage
+__device__ __forceinline__ void issue_class_tile(const ClassArgs& a, const TileRec& t0, const TileRec& t1, unsigned char* st,
+                                                 unsigned long long* bar, StageDesc& sd, unsigned n_consumers) {
     const unsigned long long vb = t0.val_begin & ~1ull, ib = t0.id_begin & ~3ull;
     const unsigned b_val = round16((unsigned)(t1.val_begin - vb) * 8u);
     const unsigned b_ids = round16((unsigned)(t1.id_begin - ib) * 4u);
@@ -535,7 +553,8 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
 // it waits on a stage's "empty" barrier (one arrival per consumer warp) and issues the next tile's bulk copies on its
 // "full" barrier.  Consumers wait for "full", take the batches whose global index is congruent to their warp index
 // (batches of a tile have similar shape, so the static assignment is balanced and costs no atomics), arrive on "empty".
-template <int W, int U>
+// PROF: wait accounting into a.wait_ns (profiling on); the kernel without it has no timer reads around the waits
+template <int W, int U, bool PROF>
 __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const ClassArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ClassSmem<W>& sm = *reinterpret_cast<ClassSmem<W>*>(smem_raw);
@@ -543,14 +562,17 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
     const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     unsigned long long t_start = 0;
     if (tid == 0) {
-        asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_start));
+        t_start = global_ns();
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&sm.full_bar[s], 1);
             mbar_init(&sm.empty_bar[s], W);
         }
+        sm.wait[0] = sm.wait[1] = 0;
         fence_barrier_init();
     }
     __syncthreads();
+    unsigned long long waited = 0;
+    unsigned long long* const wacc = PROF ? &waited : nullptr;
     // tiles strided by the grid: neighbouring tiles hold batches of similar shape (the stream is sorted by degree), so
     // every CTA sees the same mix
     const unsigned k_first = blockIdx.x, k_step = gridDim.x, k_end = a.n_tiles;
@@ -560,18 +582,19 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
             unsigned it = 0;
             for (unsigned long long k = k_first; k < k_end; k += k_step, ++it) {
                 const int s = it % kStages;
+                const TileRec t0 = a.tile[k], t1 = a.tile[k + 1];  // in flight while the stage is still in use
                 if (it >= (unsigned)kStages) {
-                    mbar_wait(&sm.empty_bar[s], ((it / kStages) - 1u) & 1u);
+                    mbar_wait_timed(&sm.empty_bar[s], ((it / kStages) - 1u) & 1u, wacc);
                     fence_proxy_async();  // the consumers' generic-proxy reads precede the async-proxy refill
                 }
-                issue_class_tile(a, (unsigned)k, sm.stage[s], &sm.full_bar[s], sm.sd[s], W);
+                issue_class_tile(a, t0, t1, sm.stage[s], &sm.full_bar[s], sm.sd[s], W);
             }
         }
     } else {
         unsigned it = 0;
         for (unsigned long long k = k_first; k < k_end; k += k_step, ++it) {
             const int s = it % kStages;
-            mbar_wait(&sm.full_bar[s], (it / kStages) & 1u);
+            mbar_wait_timed(&sm.full_bar[s], (it / kStages) & 1u, wacc);
             const unsigned char* st = sm.stage[s];
             const StageDesc sd = sm.sd[s];
             const double* s_val = reinterpret_cast<const double*>(st);
@@ -623,6 +646,7 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
     if (lane == 0) sm.red[warp] = acc0;
+    if (wacc && lane == 0) atomicAdd(&sm.wait[warp == W ? 1 : 0], waited);
     __syncthreads();
     if (warp == 0) {
         double v = 0.0;
@@ -631,9 +655,12 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if (lane == 0 && v != 0.0) red_add_f64(a.count, v);
         if (lane == 0) {
-            unsigned long long t_end;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t_end));
-            a.cta_ns[blockIdx.x] = t_end - t_start;
+            a.cta_ns[blockIdx.x] = global_ns() - t_start;
+            if (PROF) {
+                a.wait_ns[3 * blockIdx.x] = sm.wait[0];
+                a.wait_ns[3 * blockIdx.x + 1] = sm.wait[1];
+                a.wait_ns[3 * blockIdx.x + 2] = W;
+            }
         }
     }
 }
@@ -738,6 +765,7 @@ void class_free(rsem_b200_ctx* ctx) {
     ClassLayout& L = ctx->cls;
     block_free(ctx, L.vals); block_free(ctx, L.ids); block_free(ctx, L.desc); block_free(ctx, L.tile); block_free(ctx, L.batch_first);
     block_free(ctx, L.fseg_first); block_free(ctx, L.rows); block_free(ctx, L.long_rows); block_free(ctx, L.cta_ns);
+    block_free(ctx, L.wait_ns);
     L = ClassLayout{};
 }
 
@@ -945,11 +973,6 @@ int class_build(rsem_b200_ctx* ctx) {
     sc.keep(rows_s);
     L.rows = rows_s;
     L.R = R;
-    // measured on C3 (ms per round): 512 threads x 128 registers, two rows in flight per lane: 2.27; 1024 x 64, one row: 2.49
-    L.threads = 512;
-    if (const char* e = getenv("RSEM_B200_CLASS_THREADS")) {  // tuning knob: 512, 513 (3 rows in flight), 544, 640, 768, 1024
-        L.threads = atoi(e);
-    }
     L.built = true;
     L.vals_epoch = 0;
     ctx->launches += 20;
@@ -988,25 +1011,26 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
             RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.cta_ns), (size_t)ctx->sm_count * sizeof(unsigned long long)));
         }
         a.cta_ns = reinterpret_cast<unsigned long long*>(L.cta_ns);
+        if (ctx->profiling && !L.wait_ns) {
+            RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.wait_ns), (size_t)ctx->sm_count * 3 * sizeof(unsigned long long)));
+        }
+        a.wait_ns = ctx->profiling ? reinterpret_cast<unsigned long long*>(L.wait_ns) : nullptr;
+        L.last_profiled = ctx->profiling;
         unsigned grid = (unsigned)ctx->sm_count;
         if (grid > L.n_tiles) grid = L.n_tiles;
         L.last_grid = grid;
-        // consumer warps x rows in flight per lane
-        switch (L.threads) {
-#define RB_CLASS_LAUNCH(W, U)                                                                                   \
-    {                                                                                                           \
-        auto kern = estep_class_kernel<W, U>;                                                                   \
-        const size_t smem = sizeof(ClassSmem<W>);                                                               \
-        RB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));            \
-        kern<<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);                                                     \
-    }
-            case 1024: RB_CLASS_LAUNCH(31, 1) break;
-            case 768: RB_CLASS_LAUNCH(23, 2) break;
-            case 640: RB_CLASS_LAUNCH(19, 2) break;
-            case 544: RB_CLASS_LAUNCH(16, 2) break;
-            case 513: RB_CLASS_LAUNCH(15, 3) break;
-            default: RB_CLASS_LAUNCH(15, 2) break;
-#undef RB_CLASS_LAUNCH
+        // 11 consumer warps x 2 rows in flight per lane: a tile holds ~11 batches at C3, so with one batch per warp
+        // and tile no warp idles, and 384 threads leave 167 registers per thread (no spills).  Measured on C3 (H100
+        // 80GB HBM3, 700 W, ms per round): 11 warps 3.51-3.54, 11 warps x 3 rows 3.56, 15 warps (128 registers,
+        // spills) 3.81-3.84, 16 / 19 / 23 / 31 warps 4.18-5.80.
+        constexpr int W = 11, U = 2;
+        const size_t smem = sizeof(ClassSmem<W>);
+        if (ctx->profiling) {
+            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            estep_class_kernel<W, U, true><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
+        } else {
+            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            estep_class_kernel<W, U, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         }
         RB_CUDA(cudaGetLastError());
         ctx->launches++;
