@@ -237,13 +237,16 @@ int rsem_b200_set_estep_variant(rsem_b200_ctx* ctx, int32_t variant);
 
 /* Equivalence-class layout the frozen-conprb rounds run on (derived from the hit matrix on first use; reads with
  * identical transcript lists - the reference has no counterpart, it walks HitContainer row by row, EM.cpp:199-244).
- * out[8] = { built (0/1), rows in the layout, rows handled by the long-row launch, segments, batches, tiles,
- *            staged doubles (conprb + ncpv), staged ids }.  Streamed bytes per round = 8 out[6] + 4 out[7] + 16 out[4]. */
-int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 8 */);
-/* Busy time (ns, %globaltimer) of every persistent CTA in the latest class-layout E-step launch: the evidence for
- * the segmented reduction's load balance on skewed matrices (BASELINE configs[4]).  *n = CTAs written (<= cap).   */
+ * out[9] = { built (0/1), rows in the layout, rows handled by the long-row launch, segments, batches, tiles,
+ *            staged doubles (conprb + ncpv), staged ids, tiles of the main launch }.  Streamed bytes per round =
+ *            8 out[6] + 4 out[7] + 16 out[4].  Tiles [0, out[8]) hold the rows of at most 127 hits; the other
+ *            out[5] - out[8] tiles (rows of 128..2047 hits) run in a second launch.                                 */
+int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 9 */);
+/* Busy time (ns, %globaltimer) of every persistent CTA in the latest class-layout E-step launch over the main tiles
+ * (see rsem_b200_class_layout_info): the evidence for the segmented reduction's load balance on skewed matrices
+ * (BASELINE configs[4]).  *n = CTAs written (<= cap); 0 when the layout has no main tiles.                         */
 int rsem_b200_estep_cta_times(rsem_b200_ctx* ctx, uint64_t* out_ns, int32_t cap, int32_t* n);
-/* Where the class-layout E-step's time went in its latest launch with profiling on (rsem_b200_set_profiling):
+/* Where the class-layout E-step's time went in its latest main launch with profiling on (rsem_b200_set_profiling):
  * out_ns[3 i .. 3 i + 2] = { ns the consumer warps of CTA i spent blocked on staged data (summed over the warps),
  * ns a separate copy-issuing warp spent blocked on a free stage (0 when the consumer warps issue their own copies),
  * consumer warps of CTA i }.  *n = CTAs written (<= cap); 0 when the latest launch ran without profiling.          */

@@ -45,12 +45,15 @@ constexpr unsigned long long kOff48 = (1ull << 48) - 1, kOff40 = (1ull << 40) - 
 
 // A row of degree d has d + 1 columns: its d hits and the noise entry (theta[0] * ncpv, EM.cpp:210-213), which is
 // stored and processed as the last column.  Lanes per segment (G) and register slots per lane (S) from the column
-// count w: S * G >= w up to w = 128.
+// count w: S * G >= w up to w = 128.  Wider rows (G = 32, S = 4 plus a loop over the columns beyond 128) are
+// configuration kTailCfg; they run in a launch of their own so that configurations 0-11 carry no code for them.
+constexpr unsigned kTailCfg = 12;
 __host__ __device__ __forceinline__ unsigned group_of_deg(unsigned d) {
     const unsigned w = d + 1u;
     return w <= 4 ? 1u : w <= 8 ? 2u : w <= 16 ? 4u : w <= 32 ? 8u : w <= 64 ? 16u : 32u;
 }
-__host__ __device__ __forceinline__ unsigned cfg_of_deg(unsigned d) {  // 2 * log2(G) + (S == 4)
+__host__ __device__ __forceinline__ unsigned cfg_of_deg(unsigned d) {  // 2 * log2(G) + (S == 4), or kTailCfg
+    if (d + 1u > 128u) return kTailCfg;
     const unsigned G = group_of_deg(d);
     const unsigned lg = G == 1 ? 0u : G == 2 ? 1u : G == 4 ? 2u : G == 8 ? 3u : G == 16 ? 4u : 5u;
     return 2u * lg + (d + 1u > 3u * G ? 1u : 0u);
@@ -268,18 +271,40 @@ __global__ void cls_batch_desc_kernel(const unsigned* __restrict__ key2s, const 
     desc[b] = o;
 }
 
-// first batch b with cum(b) >= k W, cum(b) = 8 val_off[b] + 4 id_off[b] + 16 b (bytes staged before batch b)
+__device__ __forceinline__ unsigned long long staged_before(const unsigned long long* __restrict__ val_off,
+                                                            const unsigned long long* __restrict__ id_off, unsigned long long b) {
+    return 8ull * val_off[b] + 4ull * id_off[b] + 16ull * b;  // bytes staged before batch b
+}
+
+// one thread: out = {first batch of configuration kTailCfg (n_batches if none), bytes staged before it}.  Batches are
+// sorted by degree, so the kTailCfg batches are a suffix of the stream.
+__global__ void cls_tail_start_kernel(const unsigned* __restrict__ key2s, const unsigned* __restrict__ batch_first,
+                                      const unsigned long long* __restrict__ val_off, const unsigned long long* __restrict__ id_off,
+                                      unsigned n_batches, unsigned long long* out) {
+    unsigned lo = 0, hi = n_batches;
+    while (lo < hi) {
+        const unsigned mid = (lo + hi) >> 1;
+        if (cfg_of_deg(key2s[batch_first[mid]] >> 8) != kTailCfg) lo = mid + 1;
+        else hi = mid;
+    }
+    out[0] = lo;
+    out[1] = staged_before(val_off, id_off, lo);
+}
+
+// tiles of the batch range [b_lo, b_hi): bound[k] = first batch b in it with staged_before(b) >= base + k W, where
+// base = staged_before(b_lo); bound[n_raw] = b_hi
 __global__ void cls_tile_bounds_kernel(const unsigned long long* __restrict__ val_off,
-                                       const unsigned long long* __restrict__ id_off, unsigned n_batches,
-                                       unsigned long long W, unsigned long long n_raw, unsigned long long* bound) {
+                                       const unsigned long long* __restrict__ id_off, unsigned b_lo, unsigned b_hi,
+                                       unsigned long long base, unsigned long long W, unsigned long long n_raw,
+                                       unsigned long long* bound) {
     const unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k > n_raw) return;
-    if (k == n_raw) { bound[k] = n_batches; return; }
-    const unsigned long long target = k * W;
-    unsigned long long lo = 0, hi = n_batches;  // val_off / id_off have n_batches + 1 entries
+    if (k == n_raw) { bound[k] = b_hi; return; }
+    const unsigned long long target = base + k * W;
+    unsigned long long lo = b_lo, hi = b_hi;  // val_off / id_off have n_batches + 1 entries
     while (lo < hi) {
         const unsigned long long mid = (lo + hi) >> 1;
-        if (8ull * val_off[mid] + 4ull * id_off[mid] + 16ull * mid < target) lo = mid + 1;
+        if (staged_before(val_off, id_off, mid) < target) lo = mid + 1;
         else hi = mid;
     }
     bound[k] = lo;
@@ -362,7 +387,7 @@ struct ClassArgs {
     const double* theta;
     double* count;
     const int* done_flag;
-    unsigned long long* cta_ns;  // per-CTA busy time of this launch (globaltimer, ns): load-balance evidence
+    unsigned long long* cta_ns;  // per-CTA busy time of this launch (globaltimer, ns): load-balance evidence; or nullptr
     unsigned long long* wait_ns;  // profiling only (else nullptr): per CTA {consumer ns blocked on data, producer ns
                                   // blocked on a free stage, consumer warps}
 };
@@ -437,10 +462,11 @@ __device__ __forceinline__ double fast_rcp(double x) {
 }
 
 // U rows of a batch at once.  ROWS_OK: all U rows exist (main loop) - otherwise rows >= n_left are idle (remainder).
-template <int G, int S, int U, bool ROWS_OK>
+// TAIL: the rows have more than G * S = 128 columns (configuration kTailCfg); the rest are walked from shared memory.
+template <int G, int S, int U, bool ROWS_OK, bool TAIL>
 __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsigned row_stride, unsigned n_left,
                                            const double (&th)[S], const bool (&col_ok)[S], const unsigned (&coff)[S],
-                                           double (&acc)[S], bool tail, unsigned g, unsigned w, unsigned nsb, unsigned d,
+                                           double (&acc)[S], unsigned g, unsigned w, unsigned nsb, unsigned d,
                                            const int* __restrict__ bi, unsigned ids_stride, unsigned ids_gi, bool seg_ok,
                                            const double* __restrict__ theta, double* count, double& acc0) {
     double x[U][S], part[U];
@@ -460,7 +486,7 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
         if (S == 4) part[u] = (x[u][0] + x[u][1]) + (x[u][2] + x[u][3]);
         else part[u] = (x[u][0] + x[u][1]) + x[u][2];
     }
-    if (tail && seg_ok) {  // columns beyond G * S (rows with more than 127 hits): not kept in registers
+    if (TAIL && seg_ok) {  // columns beyond G * S (rows with more than 127 hits): not kept in registers
         for (unsigned c = g + G * S; c < w; c += G) {
             const double thc = __ldg(theta + (c < d ? bi[c * ids_stride + ids_gi] : 0));
 #pragma unroll
@@ -480,7 +506,7 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
         const double inv = part[u] >= kEpsilon ? fast_rcp(part[u]) : 0.0;  // idle rows: part = 0 -> inv = 0
 #pragma unroll
         for (int q = 0; q < S; ++q) acc[q] += x[u][q] * inv;
-        if (tail && seg_ok && (ROWS_OK || (unsigned)u < n_left)) {
+        if (TAIL && seg_ok && (ROWS_OK || (unsigned)u < n_left)) {
             for (unsigned c = g + G * S; c < w; c += G) {
                 const int tt = c < d ? bi[c * ids_stride + ids_gi] : 0;
                 double f = __ldg(theta + tt) * cr[u * row_stride + c * nsb];
@@ -497,7 +523,7 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
 // gi: ids and theta are loaded once, the rows are walked U at a time (instruction-level parallelism across the
 // load -> product -> row sum -> reciprocal chain), the normalised weights are summed per lane and leave as ONE
 // reduction per transcript and segment.  The noise column's sum stays in the thread (count[0] is flushed per CTA).
-template <int G, int S, int U>
+template <int G, int S, int U, bool TAIL>
 __device__ __forceinline__ double process_batch(const double* __restrict__ bv, const int* __restrict__ bi, unsigned d,
                                                 unsigned n, unsigned nsb, bool same, const double* __restrict__ theta,
                                                 double* count, unsigned lane) {
@@ -524,15 +550,14 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
     }
     const double* con = bv + gi;  // value (r, c) of this lane's segment at con[(r w + c) nsb]
     const unsigned row_stride = w * nsb;
-    const bool tail = w > (unsigned)(G * S);  // only possible for G = 32
     double acc0 = 0.0;
     unsigned r = 0;
     for (; r + U <= n; r += U)
-        batch_rows<G, S, U, true>(con + (unsigned long long)r * row_stride, row_stride, U, th, col_ok, coff, acc, tail, g, w, nsb, d,
-                                  bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
+        batch_rows<G, S, U, true, TAIL>(con + (unsigned long long)r * row_stride, row_stride, U, th, col_ok, coff, acc, g, w, nsb, d,
+                                        bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
     if (U > 1 && r < n)
-        batch_rows<G, S, U, false>(con + (unsigned long long)r * row_stride, row_stride, n - r, th, col_ok, coff, acc, tail, g, w, nsb,
-                                   d, bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
+        batch_rows<G, S, U, false, TAIL>(con + (unsigned long long)r * row_stride, row_stride, n - r, th, col_ok, coff, acc, g, w,
+                                         nsb, d, bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
     if (same && P > 1) {  // every segment of the batch adds to the same transcripts: fold them first
 #pragma unroll
         for (int q = 0; q < S; ++q) {
@@ -553,8 +578,9 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
 // it waits on a stage's "empty" barrier (one arrival per consumer warp) and issues the next tile's bulk copies on its
 // "full" barrier.  Consumers wait for "full", take the batches whose global index is congruent to their warp index
 // (batches of a tile have similar shape, so the static assignment is balanced and costs no atomics), arrive on "empty".
-// PROF: wait accounting into a.wait_ns (profiling on); the kernel without it has no timer reads around the waits
-template <int W, int U, bool PROF>
+// PROF: wait accounting into a.wait_ns (profiling on); the kernel without it has no timer reads around the waits.
+// TAIL: the tiles hold only configuration-kTailCfg batches (rows with more than 127 hits), else none of them.
+template <int W, int U, bool TAIL, bool PROF>
 __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const ClassArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ClassSmem<W>& sm = *reinterpret_cast<ClassSmem<W>*>(smem_raw);
@@ -623,19 +649,23 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
                                sd.id_base, sd.first_batch_mod, bd.w0, bd.w1);
                 }
 #endif
-                switch (cfg) {
-                    case 0: acc0 += process_batch<1, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 1: acc0 += process_batch<1, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 2: acc0 += process_batch<2, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 3: acc0 += process_batch<2, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 4: acc0 += process_batch<4, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 5: acc0 += process_batch<4, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 6: acc0 += process_batch<8, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 7: acc0 += process_batch<8, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 8: acc0 += process_batch<16, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 9: acc0 += process_batch<16, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    case 10: acc0 += process_batch<32, 3, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                    default: acc0 += process_batch<32, 4, U>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                if constexpr (TAIL) {
+                    acc0 += process_batch<32, 4, U, true>(bv, bi, d, n, nsb, same, a.theta, a.count, lane);
+                } else {
+                    switch (cfg) {
+                        case 0: acc0 += process_batch<1, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 1: acc0 += process_batch<1, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 2: acc0 += process_batch<2, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 3: acc0 += process_batch<2, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 4: acc0 += process_batch<4, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 5: acc0 += process_batch<4, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 6: acc0 += process_batch<8, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 7: acc0 += process_batch<8, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 8: acc0 += process_batch<16, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 9: acc0 += process_batch<16, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 10: acc0 += process_batch<32, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        default: acc0 += process_batch<32, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                    }
                 }
             }
             __syncwarp();  // every lane's reads of the stage are done before lane 0 releases it
@@ -655,7 +685,7 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if (lane == 0 && v != 0.0) red_add_f64(a.count, v);
         if (lane == 0) {
-            a.cta_ns[blockIdx.x] = global_ns() - t_start;
+            if (a.cta_ns) a.cta_ns[blockIdx.x] = global_ns() - t_start;
             if (PROF) {
                 a.wait_ns[3 * blockIdx.x] = sm.wait[0];
                 a.wait_ns[3 * blockIdx.x + 1] = sm.wait[1];
@@ -928,30 +958,54 @@ int class_build(rsem_b200_ctx* ctx) {
     cls_batch_desc_kernel<<<blocks_for(n_batches, 256), 256, 0, st>>>(key2_s, L.batch_first, val_off, id_off, same_class, n_batches,
                                                                      n_segs, static_cast<BatchDesc*>(L.desc));
     RB_CUDA(cudaGetLastError());
-    // ---- 4. tiles: contiguous batch ranges of <= kStageBytes staged bytes
+    // ---- 4. tiles: contiguous batch ranges of <= kStageBytes staged bytes.  The kTailCfg batches start a tile of
+    // their own: tiles [0, n_tiles_main) have none of them, the rest nothing else.
     {
+        unsigned long long* d_cut = nullptr;
+        RB_CUDA(sc.alloc(&d_cut, 2));
+        cls_tail_start_kernel<<<1, 1, 0, st>>>(key2_s, L.batch_first, val_off, id_off, n_batches, d_cut);
+        RB_CUDA(cudaGetLastError());
+        unsigned long long cut[2] = {0, 0};  // first kTailCfg batch, bytes staged before it
+        RB_CUDA(cudaMemcpyAsync(cut, d_cut, sizeof(cut), cudaMemcpyDeviceToHost, st));
+        RB_CUDA(cudaStreamSynchronize(st));
         const unsigned long long W = kStageBytes - max_batch_bytes - 128u;
         const unsigned long long total = 8ull * totals[0] + 4ull * totals[1] + 16ull * n_batches;
-        const unsigned long long n_raw = total / W + 1;
+        const unsigned b_tail = (unsigned)cut[0];
+        const unsigned piece_b[3] = {0u, b_tail, n_batches};
+        const unsigned long long piece_bytes[3] = {0ull, cut[1], total};
+        unsigned long long n_raw[2] = {0, 0};
+        for (int p = 0; p < 2; ++p)
+            if (piece_b[p] < piece_b[p + 1]) n_raw[p] = (piece_bytes[p + 1] - piece_bytes[p]) / W + 1;
         unsigned long long *bound = nullptr, *bound_u = nullptr;
         unsigned long long* d_n = nullptr;
-        RB_CUDA(sc.alloc(&bound, n_raw + 1));
-        RB_CUDA(sc.alloc(&bound_u, n_raw + 1));
+        RB_CUDA(sc.alloc(&bound, n_raw[0] + n_raw[1] + 2));
+        RB_CUDA(sc.alloc(&bound_u, n_raw[0] + n_raw[1] + 2));
         RB_CUDA(sc.alloc(&d_n, 1));
-        cls_tile_bounds_kernel<<<blocks_for(n_raw + 1, 256), 256, 0, st>>>(val_off, id_off, n_batches, W, n_raw, bound);
-        RB_CUDA(cudaGetLastError());
         size_t need3 = 0;
-        cub::DeviceSelect::Unique(nullptr, need3, bound, bound_u, d_n, (long long)n_raw + 1, st);
+        cub::DeviceSelect::Unique(nullptr, need3, bound, bound_u, d_n, (long long)std::max(n_raw[0], n_raw[1]) + 1, st);
         if (need3 > tmp_bytes) {
             sc.release(tmp);
             RB_CUDA(sc.alloc(reinterpret_cast<unsigned char**>(&tmp), need3));
             tmp_bytes = need3;
         }
-        need3 = tmp_bytes;
-        RB_CUDA(cub::DeviceSelect::Unique(tmp, need3, bound, bound_u, d_n, (long long)n_raw + 1, st));
+        // each piece's bounds run from its first batch to its last + 1; the main piece's last bound is the tail
+        // piece's first, so the tail piece's bounds overwrite it
         unsigned long long n_bounds = 0;
-        RB_CUDA(cudaMemcpyAsync(&n_bounds, d_n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        RB_CUDA(cudaStreamSynchronize(st));
+        L.n_tiles_main = 0;
+        for (int p = 0; p < 2; ++p) {
+            if (!n_raw[p]) continue;
+            cls_tile_bounds_kernel<<<blocks_for(n_raw[p] + 1, 256), 256, 0, st>>>(val_off, id_off, piece_b[p], piece_b[p + 1],
+                                                                                  piece_bytes[p], W, n_raw[p], bound);
+            RB_CUDA(cudaGetLastError());
+            const unsigned long long at = n_bounds ? n_bounds - 1 : 0;
+            need3 = tmp_bytes;
+            RB_CUDA(cub::DeviceSelect::Unique(tmp, need3, bound, bound_u + at, d_n, (long long)n_raw[p] + 1, st));
+            unsigned long long n = 0;
+            RB_CUDA(cudaMemcpyAsync(&n, d_n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            RB_CUDA(cudaStreamSynchronize(st));
+            n_bounds = at + n;
+            if (p == 0) L.n_tiles_main = (unsigned)(n_bounds - 1);
+        }
         L.n_tiles = (unsigned)(n_bounds - 1);
         RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.tile), n_bounds * sizeof(TileRec)));
         cls_tile_rec_kernel<<<blocks_for(n_bounds, 256), 256, 0, st>>>(bound_u, val_off, id_off, n_bounds, static_cast<TileRec*>(L.tile));
@@ -997,16 +1051,17 @@ int class_fill_vals(rsem_b200_ctx* ctx) {
 
 int class_launch_estep(rsem_b200_ctx* ctx) {
     ClassLayout& L = ctx->cls;
-    if (L.n_tiles) {
-        ClassArgs a;
-        a.vals = L.vals;
-        a.ids = L.ids;
-        a.desc = static_cast<const BatchDesc*>(L.desc);
+    ClassArgs a;
+    a.vals = L.vals;
+    a.ids = L.ids;
+    a.desc = static_cast<const BatchDesc*>(L.desc);
+    a.theta = ctx->theta;
+    a.count = ctx->k2_target;
+    a.done_flag = ctx->done_flag;
+    L.last_grid = 0;
+    if (L.n_tiles_main) {  // rows of <= 127 hits; the per-CTA busy and wait times come from this launch
         a.tile = static_cast<const TileRec*>(L.tile);
-        a.n_tiles = L.n_tiles;
-        a.theta = ctx->theta;
-        a.count = ctx->k2_target;
-        a.done_flag = ctx->done_flag;
+        a.n_tiles = L.n_tiles_main;
         if (!L.cta_ns) {
             RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.cta_ns), (size_t)ctx->sm_count * sizeof(unsigned long long)));
         }
@@ -1016,22 +1071,39 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         }
         a.wait_ns = ctx->profiling ? reinterpret_cast<unsigned long long*>(L.wait_ns) : nullptr;
         L.last_profiled = ctx->profiling;
-        unsigned grid = (unsigned)ctx->sm_count;
-        if (grid > L.n_tiles) grid = L.n_tiles;
+        const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
         L.last_grid = grid;
-        // 11 consumer warps x 2 rows in flight per lane: a tile holds ~11 batches at C3, so with one batch per warp
-        // and tile no warp idles, and 384 threads leave 167 registers per thread (no spills).  Measured on C3 (H100
-        // 80GB HBM3, 700 W, ms per round): 11 warps 3.51-3.54, 11 warps x 3 rows 3.56, 15 warps (128 registers,
-        // spills) 3.81-3.84, 16 / 19 / 23 / 31 warps 4.18-5.80.
-        constexpr int W = 11, U = 2;
+        // 15 consumer warps x 2 rows in flight per lane (102 registers, no spills).  Without the tail code more warps
+        // fit and hide more of a batch's latency (ids -> theta gather -> values -> row sums); 18 warps are no faster.
+        // Measured on H100 80GB HBM3 at 700 W, ms per round, median of 3 alternating runs in one process:
+        //   consumer warps x rows:  11x2   11x3   11x4   14x2   14x3   14x4   15x2   15x3   15x4   18x2   18x3   18x4
+        //   C3                      3.505  3.460  3.446  3.389  3.396  3.410  3.389  3.394  3.397  3.387  3.483  3.697
+        //   C2                      0.373  0.373  0.376  0.371  0.372  0.374  0.372  0.372  0.374  0.370  0.371  0.405
+        //   C5                      8.167  8.292  8.589  7.952  8.044  8.294  7.813  7.977  8.187  7.818  7.895  8.302
+        // (18 x 3 and 18 x 4 spill.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
+        // registers), in a separate process on the same card: C3 3.519, C2 0.373, C5 8.579.
+        constexpr int W = 15, U = 2;
         const size_t smem = sizeof(ClassSmem<W>);
         if (ctx->profiling) {
-            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            estep_class_kernel<W, U, true><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
+            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            estep_class_kernel<W, U, false, true><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         } else {
-            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            estep_class_kernel<W, U, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
+            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            estep_class_kernel<W, U, false, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         }
+        RB_CUDA(cudaGetLastError());
+        ctx->launches++;
+    }
+    if (L.n_tiles > L.n_tiles_main) {  // rows of 128..kLongDeg hits (none at C2 / C3, a third of the hits at C5)
+        a.tile = static_cast<const TileRec*>(L.tile) + L.n_tiles_main;
+        a.n_tiles = L.n_tiles - L.n_tiles_main;
+        a.cta_ns = nullptr;
+        a.wait_ns = nullptr;
+        const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
+        constexpr int W = 11, U = 2;
+        const size_t smem = sizeof(ClassSmem<W>);
+        RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        estep_class_kernel<W, U, true, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         RB_CUDA(cudaGetLastError());
         ctx->launches++;
     }

@@ -132,6 +132,7 @@ struct ClassLayout {
     bool built = false;
     uint64_t vals_epoch = 0;        // conprb epoch the value stream was gathered at (0 = never)
     uint32_t n_rows = 0, n_long = 0, n_segs = 0, n_batches = 0, n_tiles = 0, R = 0;
+    uint32_t n_tiles_main = 0;      // tiles [0, n_tiles_main): rows of <= 127 hits; the rest: longer rows (own launch)
     uint64_t n_vals = 0, n_ids = 0;
     double* vals = nullptr;         // per batch: ncpv [row][segment], then conprb [(row, column)][segment]
     int32_t* ids = nullptr;         // per batch: transcript ids [column][segment] (or [column] for a one-class batch)
@@ -141,8 +142,8 @@ struct ClassLayout {
     uint32_t* fseg_first = nullptr;   // first sorted row position of every segment (final order)
     uint32_t* rows = nullptr;         // sorted position -> original row
     uint32_t* long_rows = nullptr;    // original rows with more than kLongDeg hits
-    uint64_t* cta_ns = nullptr;       // per-CTA busy time (ns) of the latest class-kernel launch
-    uint64_t* wait_ns = nullptr;      // per-CTA wait accounting of the latest profiled launch (3 entries per CTA)
+    uint64_t* cta_ns = nullptr;       // per-CTA busy time (ns) of the latest class-kernel launch over the main tiles
+    uint64_t* wait_ns = nullptr;      // per-CTA wait accounting of the latest profiled main launch (3 entries per CTA)
     uint32_t last_grid = 0;
     bool last_profiled = false;       // the latest class-kernel launch ran with profiling on (wait_ns is current)
 };
