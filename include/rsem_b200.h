@@ -221,6 +221,69 @@ int rsem_b200_gibbs_upload(rsem_b200_ctx* ctx, uint64_t N1, uint64_t E, int32_t 
                            const int32_t* sid, const double* conprb);
 int rsem_b200_gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* params, rsem_b200_gibbs_out* out);
 
+typedef struct rsem_b200_sim_stats rsem_b200_sim_stats;
+
+/* ---- read simulation (rsem-simulate-reads, simulation.cpp:86-130) ------------------------------
+ * All tables are the cumulative arrays the reference's startSimulation builds, in its layout:
+ *   theta_cdf       M + 1: prefix sums of theta (SingleModel.h / PairedEndQModel.h startSimulation)
+ *   gld, mld        LenDist (LenDist.h:255-262 samples cdf + 1); mld only when the model has one
+ *   rspd_cdf        estRSPD only: transcript i's fullLen values evalCDF(j + 1, fullLen) at rspd_off[i]
+ *                   (RSPD.h:182-193); rspd_off has M + 2 entries
+ *   qd_*_cdf        QualDist, Q models: 100 and 100 x 100 (QualDist.h:116-130)
+ *   profile_cdf     pro_rows x 5 x 5: QProfile (100 rows, QProfile.h:151-193) or Profile (proLen rows,
+ *                   Profile.h:163-205), after the reference's zero-row repair
+ *   noise_cdf       NoiseQProfile 100 x 5 (NoiseQProfile.h:153-166) or NoiseProfile 5 (NoiseProfile.h:137-144)
+ *   seq / seq_off   forward-strand base codes 0..4 (A C G T N) per transcript, as upload_refs takes them
+ * exact_body = 1 when a reachable table row sums to 0 (simul.h:29-32 then draws a second word), so the number of
+ * words an attempt takes depends on the drawn qualities.  With 0 the attempt lengths are computed from the first
+ * draws only; a wrong 0 gives wrong reads.
+ * window_words: stream words per device window (0 = default); small values are for tests.                  */
+typedef struct rsem_b200_sim_params {
+    int32_t model_type;  /* 0 SingleModel, 1 SingleQModel, 2 PairedEndModel, 3 PairedEndQModel */
+    int32_t M;
+    uint32_t seed;       /* boost::mt19937(seed), simul.h:11 */
+    int32_t exact_body;
+    uint64_t N;          /* reads to simulate */
+    uint64_t window_words;
+    const double* theta_cdf;
+    double ori_prob0;    /* Orientation prob[0] (Orientation.h:36) */
+    rsem_b200_lendist gld, mld; /* pdf is not read */
+    int32_t has_mld;
+    int32_t est_rspd;
+    const uint64_t* rspd_off;
+    const double* rspd_cdf;
+    const double* qd_init_cdf;
+    const double* qd_tran_cdf;
+    int32_t pro_rows;
+    int32_t reserved;
+    const double* profile_cdf;
+    const double* noise_cdf;
+    const uint64_t* seq_off;   /* M + 2 */
+    const uint8_t* seq;
+    const int32_t* tot_len;    /* M + 1 */
+    const int32_t* full_len;   /* M + 1 */
+} rsem_b200_sim_params;
+
+/* uploads the tables and seeds the stream (simulation.cpp:117-120, simul.h:11) */
+int rsem_b200_sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* params);
+/* the next chunk of reads, in order (simulation.cpp:121-126): *n_reads reads as the text of the read file(s)
+ * (SingleRead(Q)::write, PairedEndRead(Q)::write: mate 1 in text[0], mate 2 in text[1]).  The buffers belong to the
+ * context and stay valid until the second following call, so a caller can write one chunk while it asks for the
+ * next.  *n_reads == 0: all N reads were returned.                                                          */
+int rsem_b200_sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
+/* device time per phase, summed over the windows (CUDA events) */
+typedef struct rsem_b200_sim_stats {
+    double generate_ms;  /* mt19937 stream generation (on its own stream, overlapped with the other phases) */
+    double resolve_ms;   /* attempt lengths + chain resolution                                           */
+    double reads_ms;     /* read heads, offsets, text formatting                                         */
+    double copy_ms;      /* read text to the host                                                        */
+    uint64_t words;      /* stream words generated                                                       */
+    uint64_t windows;
+} rsem_b200_sim_stats;
+/* counts[sid] of the simulated reads (M + 1), the number of failed attempts ("resimulation") and, when stats is not
+ * NULL, the phase times; frees the state                                                                     */
+int rsem_b200_sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
+
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);

@@ -1,7 +1,8 @@
 """In-tree build of every native artefact (called by __graft_entry__.build()).
 
   rsem_b200/librsem_b200.so   CUDA kernels + C ABI, sm_90a only
-  bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments   C++ drop-in executables (link the .so)
+  bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments, bin/rsem-simulate-reads
+                              C++ drop-in executables (link the .so)
   tools/gen_dataset           synthetic intermediate-file generator (tooling)
   oracle/librsem_oracle.so    CPU restatement (test infrastructure)
   oracle/_ref/*               reference binaries, only when /root/reference is present
@@ -48,13 +49,24 @@ def build_host(force: bool = False):
     common = sorted(glob.glob(os.path.join(HOST, "*.cpp")))
     mains = [s for s in common if os.path.basename(s).startswith("main_")]
     shared = [s for s in common if s not in mains]
-    deps = common + glob.glob(os.path.join(HOST, "*.hpp")) + [os.path.join(ROOT, "include", "rsem_b200.h")]
+    # the simulator's tables are built in a file compiled with the reference's flags for simulation.cpp (-O3 -ffast-math,
+    # reference Makefile:39,72-73), so that they carry the same bits
+    ffm = sorted(glob.glob(os.path.join(HOST, "ffm", "*.cpp")))
+    deps = common + ffm + glob.glob(os.path.join(HOST, "*.hpp")) + [os.path.join(ROOT, "include", "rsem_b200.h")]
+    ffm_objs = []
+    for src in ffm:
+        obj = os.path.join(ROOT, "build", "host", os.path.basename(src)[:-4] + ".o")
+        os.makedirs(os.path.dirname(obj), exist_ok=True)
+        if force or _newer(obj, deps):
+            _run(["g++", "-O3", "-ffast-math", "-std=c++17", "-Wall", "-I", os.path.join(ROOT, "include"), "-c", "-o", obj, src])
+        ffm_objs.append(obj)
     for m in mains:
-        name = {"main_em.cpp": "rsem-run-em", "main_gibbs.cpp": "rsem-run-gibbs",
+        name = {"main_em.cpp": "rsem-run-em", "main_gibbs.cpp": "rsem-run-gibbs", "main_simulate.cpp": "rsem-simulate-reads",
                 "main_selftest.cpp": "rsem-b200-host-selftest", "main_parse.cpp": "rsem-parse-alignments"}[os.path.basename(m)]
         out = os.path.join(ROOT, "bin", name)
+        extra = ffm_objs if name == "rsem-simulate-reads" else []
         if force or _newer(out, deps + [os.path.join(ROOT, "rsem_b200", "librsem_b200.so")]):
-            _run(["g++", "-O2", "-std=c++17", "-Wall", "-pthread", "-I", os.path.join(ROOT, "include"), "-o", out, m, *shared,
+            _run(["g++", "-O2", "-std=c++17", "-Wall", "-pthread", "-I", os.path.join(ROOT, "include"), "-o", out, m, *shared, *extra,
                   "-L", os.path.join(ROOT, "rsem_b200"), "-lrsem_b200", "-Wl,-rpath,$ORIGIN/../rsem_b200",
                   "-static-libstdc++", "-static-libgcc", "-lz"])
 
@@ -75,6 +87,7 @@ def build_tools(force: bool = False):
 def build_oracle():
     # building the checker is not using it; `make ref` is a no-op when /root/reference is absent
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "all"])
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "-f", "simulate.mk"])
 
 
 def build_all(force: bool = False):

@@ -53,6 +53,22 @@ class GibbsOut(C.Structure):
                 ("sum_fpkm", C.POINTER(C.c_double)), ("sum_gene_c2", C.POINTER(C.c_double))]
 
 
+class SimParams(C.Structure):
+    _fields_ = [("model_type", C.c_int32), ("M", C.c_int32), ("seed", C.c_uint32), ("exact_body", C.c_int32),
+                ("N", C.c_uint64), ("window_words", C.c_uint64), ("theta_cdf", C.POINTER(C.c_double)),
+                ("ori_prob0", C.c_double), ("gld", LenDist), ("mld", LenDist), ("has_mld", C.c_int32),
+                ("est_rspd", C.c_int32), ("rspd_off", C.POINTER(C.c_uint64)), ("rspd_cdf", C.POINTER(C.c_double)),
+                ("qd_init_cdf", C.POINTER(C.c_double)), ("qd_tran_cdf", C.POINTER(C.c_double)),
+                ("pro_rows", C.c_int32), ("reserved", C.c_int32), ("profile_cdf", C.POINTER(C.c_double)),
+                ("noise_cdf", C.POINTER(C.c_double)), ("seq_off", C.POINTER(C.c_uint64)),
+                ("seq", C.POINTER(C.c_uint8)), ("tot_len", C.POINTER(C.c_int32)), ("full_len", C.POINTER(C.c_int32))]
+
+
+class SimStats(C.Structure):
+    _fields_ = [("generate_ms", C.c_double), ("resolve_ms", C.c_double), ("reads_ms", C.c_double),
+                ("copy_ms", C.c_double), ("words", C.c_uint64), ("windows", C.c_uint64)]
+
+
 def _dp(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
 
@@ -77,7 +93,8 @@ SYMBOLS = [
     "rsem_b200_em_rounds", "rsem_b200_em_model_round", "rsem_b200_expected_weights", "rsem_b200_gibbs_upload",
     "rsem_b200_gibbs_run", "rsem_b200_launch_count", "rsem_b200_estep_timing", "rsem_b200_set_profiling",
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
-    "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times",
+    "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
+    "rsem_b200_sim_end",
 ]
 
 
@@ -267,6 +284,26 @@ class Context:
 
     def gibbs_run(self, params: GibbsParams, out: GibbsOut):
         self.lib.check(self.lib.dll.rsem_b200_gibbs_run(self._h, C.byref(params), C.byref(out)))
+
+    def sim_begin(self, params: SimParams):
+        """params' arrays must stay alive until sim_begin returns (they are copied to the device)"""
+        self.lib.check(self.lib.dll.rsem_b200_sim_begin(self._h, C.byref(params)))
+
+    def sim_next(self):
+        """-> (n_reads, [mate 1 text, mate 2 text]) of the next chunk; n_reads == 0 after the last one"""
+        text = (C.c_void_p * 2)()
+        nbytes = (C.c_uint64 * 2)()
+        n = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rsem_b200_sim_next(self._h, text, nbytes, C.byref(n)))
+        return n.value, [C.string_at(text[i], nbytes[i]) if text[i] else b"" for i in range(2)]
+
+    def sim_end(self, M: int):
+        """-> (counts per sid, M + 1 doubles; number of failed attempts; SimStats phase times)"""
+        counts = np.zeros(M + 1, np.float64)
+        resim = C.c_uint64(0)
+        stats = SimStats()
+        self.lib.check(self.lib.dll.rsem_b200_sim_end(self._h, _dp(counts), C.byref(resim), C.byref(stats)))
+        return counts, resim.value, stats
 
     # ---- instrumentation
     def launch_count(self) -> int:

@@ -286,6 +286,7 @@ int rsem_b200_ctx_destroy(rsem_b200_ctx* c) {
     free_reads(c);
     free_refs(c);
     free_gibbs(c);
+    sim_free(c);
     if (c->model_buf) cudaFree(c->model_buf);
     if (c->stats_buf) cudaFree(c->stats_buf);
     if (c->d_stats) cudaFree(c->d_stats);
@@ -721,6 +722,32 @@ int rsem_b200_gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_
     RB_ARG(p->n_chains >= 1 && p->chain_samples && p->chain_seeds, "bad chain parameters");
     RB_CUDA(cudaSetDevice(c->device));
     return gibbs_run(c, p, out);
+}
+
+int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
+    RB_ARG(c && p, "NULL argument");
+    RB_ARG(p->model_type >= 0 && p->model_type <= 3 && p->M >= 1, "bad model type or M");
+    RB_ARG(p->theta_cdf && p->gld.cdf && p->profile_cdf && p->noise_cdf && p->seq_off && p->seq && p->tot_len &&
+               p->full_len, "NULL table");
+    RB_ARG(p->gld.span == p->gld.ub - p->gld.lb && p->gld.span >= 1, "bad gld");
+    RB_ARG(p->model_type < 2 || p->has_mld, "paired-end models need mld");
+    RB_ARG(!p->has_mld || (p->mld.cdf && p->mld.span == p->mld.ub - p->mld.lb && p->mld.span >= 1), "bad mld");
+    RB_ARG(!p->est_rspd || (p->rspd_off && p->rspd_cdf), "estRSPD needs rspd_off / rspd_cdf");
+    RB_ARG(!(p->model_type & 1) || (p->qd_init_cdf && p->qd_tran_cdf && p->pro_rows == 100), "Q models need QualDist");
+    RB_CUDA(cudaSetDevice(c->device));
+    return sim_begin(c, p);
+}
+
+int rsem_b200_sim_next(rsem_b200_ctx* c, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {
+    RB_ARG(c && text && bytes && n_reads, "NULL argument");
+    RB_CUDA(cudaSetDevice(c->device));
+    return sim_next(c, text, bytes, n_reads);
+}
+
+int rsem_b200_sim_end(rsem_b200_ctx* c, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats) {
+    RB_ARG(c, "NULL argument");
+    RB_CUDA(cudaSetDevice(c->device));
+    return sim_end(c, counts, resim, stats);
 }
 
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {

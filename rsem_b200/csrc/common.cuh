@@ -148,6 +148,8 @@ struct ClassLayout {
     bool last_profiled = false;       // the latest class-kernel launch ran with profiling on (wait_ns is current)
 };
 
+struct SimState;  // sim_kernels.cu
+
 }  // namespace rsem_b200
 
 struct rsem_b200_ctx {
@@ -220,6 +222,7 @@ struct rsem_b200_ctx {
     rsem_b200::DevRefs refs;
 
     rsem_b200::DevGibbs gibbs;
+    rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads between sim_begin and sim_end
 
     // multi-GPU
     void* comm = nullptr;
@@ -298,5 +301,11 @@ int model_launch_update(rsem_b200_ctx* ctx);
 // gibbs_kernels.cu
 int gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out);
 int gibbs_prepare(rsem_b200_ctx* ctx, const uint64_t* row_ptr, const int32_t* sid);
+
+// sim_kernels.cu
+int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p);
+int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
+int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
+void sim_free(rsem_b200_ctx* ctx);
 
 }  // namespace rsem_b200

@@ -167,6 +167,8 @@ struct HostModel {
     void write(const std::string& path) const;   // Model::write
     // Model::read for rsem-run-gibbs: only gld and mw are needed afterwards, but the whole file is parsed
     static void read_for_gibbs(const std::string& path, int M, int& model_type, LenDistH& gld, std::vector<double>& mw);
+    // the whole .model file, every model type (rsem-simulate-reads); mw stays empty when the file has none for M
+    void read(const std::string& path, int M);
 };
 
 // ---- O(M) result math (WriteResults.h:24-104) ------------------------------------------------------
@@ -181,6 +183,9 @@ void write_results_gibbs(const std::string& ref_name, const std::string& imd_nam
                          const std::vector<double>& pme_fpkm, const std::vector<double>& pme_tpm,
                          const std::vector<double>& pve_c, const std::vector<double>& pve_c_genes,
                          const std::vector<double>& pve_c_trans);  // WriteResults.h:357-479
+void write_results_simulation(const std::string& ref_name, const std::string& out_name,
+                              const std::vector<TranscriptInfo>& tr, const std::vector<double>& eel,
+                              const std::vector<double>& counts);  // WriteResults.h:481-635
 
 // ---- alignment files for -b: SAM / BAM in, BAM out (bam.cpp; BamWriter.h, sam_utils.h, SamHeader.cpp) -----------------
 struct BamRecord {

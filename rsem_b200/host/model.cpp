@@ -547,6 +547,62 @@ void HostModel::read_for_gibbs(const std::string& path, int M, int& model_type, 
     if (mw.empty()) die("The .model file does not carry mask weights for this reference!");
 }
 
+// Model::read (SingleModel.h:356-381, SingleQModel.h:383-411, PairedEndModel.h:296-317, PairedEndQModel.h:316-343)
+void HostModel::read(const std::string& path, int M) {
+    FILE* fi = fopen(path.c_str(), "r");
+    if (!fi) die("Cannot open " + path + "! It may not exist.");
+    auto need = [&](bool ok) { if (!ok) die("Cannot parse " + path + "!"); };
+    int v;
+    need(fscanf(fi, "%d", &type) == 1 && type >= 0 && type <= 3);
+    need(fscanf(fi, "%lf", &ori[0]) == 1);  // Orientation.h:26-29
+    ori[1] = 1.0 - ori[0];
+    gld.read(fi);
+    if (paired()) { mld.read(fi); has_mld = true; }
+    else {
+        need(fscanf(fi, "%d", &v) == 1);
+        has_mld = v > 0;
+        if (has_mld) mld.read(fi);
+    }
+    need(fscanf(fi, "%d", &v) == 1);  // RSPD.h:138-167
+    mp.estRSPD = v != 0;
+    if (mp.estRSPD) need(fscanf(fi, "%d", &mp.B) == 1 && mp.B >= 1);
+    const int B = mp.estRSPD ? mp.B : 20;
+    rspd_pdf.assign(B + 2, 0.0);
+    rspd_cdf.assign(B + 2, 0.0);
+    for (int i = 1; i <= B; ++i) {
+        if (mp.estRSPD) need(fscanf(fi, "%lf", &rspd_pdf[i]) == 1);
+        else rspd_pdf[i] = 1.0 / B;
+        rspd_cdf[i] = mp.estRSPD ? rspd_cdf[i - 1] + rspd_pdf[i] : i * 1.0 / B;
+    }
+    if (hasq()) {  // QualDist.h:94-104
+        need(fscanf(fi, "%d", &v) == 1 && v == 100);
+        qd_init.assign(100, 0.0);
+        qd_tran.assign(100 * 100, 0.0);
+        for (double& d : qd_init) need(fscanf(fi, "%lf", &d) == 1);
+        for (double& d : qd_tran) need(fscanf(fi, "%lf", &d) == 1);
+    }
+    int rows, ncodes;  // QProfile.h:129-137, Profile.h:133-149
+    need(fscanf(fi, "%d %d", &rows, &ncodes) == 2 && ncodes == 5 && rows >= 0 && (!hasq() || rows == 100));
+    pro_len = hasq() ? 0 : rows;
+    profile.assign((size_t)rows * 25, 0.0);
+    for (double& d : profile) need(fscanf(fi, "%lf", &d) == 1);
+    if (hasq()) {  // NoiseQProfile.h:132-143
+        need(fscanf(fi, "%d %d", &rows, &ncodes) == 2 && rows == 100 && ncodes == 5);
+        noise_p.assign(500, 0.0);
+    } else {  // NoiseProfile.h:119-127
+        need(fscanf(fi, "%d", &ncodes) == 1 && ncodes == 5);
+        noise_p.assign(5, 0.0);
+    }
+    for (double& d : noise_p) need(fscanf(fi, "%lf", &d) == 1);
+    mw.clear();
+    if (fscanf(fi, "%d", &v) == 1 && v == M) {
+        mw.resize((size_t)M + 1);
+        for (int i = 0; i <= M; ++i) need(fscanf(fi, "%lf", &mw[i]) == 1);
+    }
+    mp.M = M;
+    fclose(fi);
+}
+
 // ---- WriteResults.h:24-104 ---------------------------------------------------------------------------------
 void calc_eel(const RefData& refs, const LenDistH& gld, std::vector<double>& eel) {
     const int lb = gld.lb, ub = gld.ub, span = gld.span;

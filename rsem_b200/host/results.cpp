@@ -232,3 +232,76 @@ void write_results_gibbs(const std::string& ref_name, const std::string& imd_nam
 }
 
 }  // namespace host
+
+namespace host {
+
+// writeResultsSimulation (WriteResults.h:481-635): one row per transcript / gene, from the simulated counts
+void write_results_simulation(const std::string& ref_name, const std::string& out_name,
+                              const std::vector<TranscriptInfo>& tr, const std::vector<double>& eel,
+                              const std::vector<double>& counts) {
+    const int M = (int)counts.size() - 1;
+    std::vector<int> gi, gt, ta;
+    load_groups(ref_name + ".grp", gi);
+    const int m = (int)gi.size() - 1;
+    const bool alleleS = load_allele_groups(ref_name, gt, ta);
+    for (int i = 1; i <= M; ++i)
+        if (!(eel[i] > kEps || counts[i] <= kEps)) die("An isoform whose effecitve length < 1.000000 got sampled!");
+
+    std::vector<double> tpm, fpkm;
+    expression_values(counts, eel, tpm, fpkm);
+    std::vector<double> tlens(M + 1, 0.0), isopct(M + 1, 0.0);
+    for (int j = 1; j <= M; ++j) tlens[j] = tr[j].length;
+    GroupAgg gene;
+    aggregate(gi, tlens, eel, counts.data(), tpm, fpkm, gene, isopct);
+
+    if (alleleS) {
+        const int m_trans = (int)ta.size() - 1;
+        std::vector<double> ta_pct(M + 1, 0.0), gt_pct(m_trans, 0.0);
+        GroupAgg trans;
+        aggregate(ta, tlens, eel, counts.data(), tpm, fpkm, trans, ta_pct);
+        for (int i = 0; i < m; ++i)
+            if (gene.tpm[i] >= kEps)
+                for (int j = gt[i]; j < gt[i + 1]; ++j) gt_pct[j] = trans.tpm[j] / gene.tpm[i];
+
+        FILE* fo = open_or_die(out_name + ".sim.alleles.results", "w");
+        fprintf(fo, "allele_id\ttranscript_id\tgene_id\tlength\teffective_length\tcount\tTPM\tFPKM\tAlleleIsoPct\tAlleleGenePct\n");
+        for (int i = 1; i <= M; ++i)
+            fprintf(fo, "%s\t%s\t%s\t%d\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\n", tr[i].seqname.c_str(),
+                    tr[i].transcript_id.c_str(), tr[i].gene_id.c_str(), tr[i].length, eel[i], counts[i], tpm[i], fpkm[i],
+                    ta_pct[i] * 1e2, isopct[i] * 1e2);
+        fclose(fo);
+
+        fo = open_or_die(out_name + ".sim.isoforms.results", "w");
+        fprintf(fo, "transcript_id\tgene_id\tlength\teffective_length\tcount\tTPM\tFPKM\tIsoPct\n");
+        for (int i = 0; i < m_trans; ++i) {
+            const TranscriptInfo& t = tr[ta[i]];
+            fprintf(fo, "%s\t%s\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\n", t.transcript_id.c_str(), t.gene_id.c_str(),
+                    trans.lens[i], trans.eels[i], trans.counts[i], trans.tpm[i], trans.fpkm[i], gt_pct[i] * 1e2);
+        }
+        fclose(fo);
+    } else {
+        FILE* fo = open_or_die(out_name + ".sim.isoforms.results", "w");
+        fprintf(fo, "transcript_id\tgene_id\tlength\teffective_length\tcount\tTPM\tFPKM\tIsoPct\n");
+        for (int i = 1; i <= M; ++i)
+            fprintf(fo, "%s\t%s\t%d\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\n", tr[i].transcript_id.c_str(), tr[i].gene_id.c_str(),
+                    tr[i].length, eel[i], counts[i], tpm[i], fpkm[i], isopct[i] * 1e2);
+        fclose(fo);
+    }
+
+    FILE* fo = open_or_die(out_name + ".sim.genes.results", "w");
+    fprintf(fo, "gene_id\ttranscript_id(s)\tlength\teffective_length\tcount\tTPM\tFPKM\n");
+    for (int i = 0; i < m; ++i) {
+        fprintf(fo, "%s\t", tr[gi[i]].gene_id.c_str());
+        std::string cur;
+        for (int j = gi[i]; j < gi[i + 1]; ++j)
+            if (cur != tr[j].transcript_id) {
+                if (cur != "") fputc(',', fo);
+                fputs(tr[j].transcript_id.c_str(), fo);
+                cur = tr[j].transcript_id;
+            }
+        fprintf(fo, "\t%.2f\t%.2f\t%.2f\t%.2f\t%.2f\n", gene.lens[i], gene.eels[i], gene.counts[i], gene.tpm[i], gene.fpkm[i]);
+    }
+    fclose(fo);
+}
+
+}  // namespace host
