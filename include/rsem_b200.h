@@ -284,6 +284,48 @@ typedef struct rsem_b200_sim_stats {
  * NULL, the phase times; frees the state                                                                     */
 int rsem_b200_sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 
+/* ---- rsem-calculate-credibility-intervals, Phase II (K8, ci_kernels.cu) ------------------------------------------------
+ * Replaces the reference's temp-file transpose (Buffer.h:41-80, calcCI.cpp:302-305) and calculate_credibility_intervals
+ * (calcCI.cpp:286-508).  The caller draws the samples (calcCI.cpp:93-164) and pushes each one's TPM row and l_bar at a
+ * fixed sample index; ci_end returns the intervals of every transcript, gene and (allele-specific references) isoform.
+ * gene_start / isoform_start are GroupInfo start arrays (1-based transcript ids, n + 1 entries, GroupInfo.h:34-53);
+ * part_gene_start are the gene ranges of the reference's Phase II threads (calcCI.cpp:402-420): the isoform sums of an
+ * allele-specific reference run on across the isoforms of one range (calcCI.cpp:308-345), so their ranges matter.
+ * threshold = nSamples - (int(confidence * nSamples - 1e-8) + 1) (calcCI.cpp:221).
+ * device_budget: bytes of device memory to use (0 = what is free less 512 MB); when the sample matrix does not fit next
+ * to the rows of the largest gene it is kept in pinned host memory and gathered block by block.                   */
+typedef struct rsem_b200_ci_params {
+    int32_t M;
+    int32_t n_genes;
+    const int32_t* gene_start;       /* n_genes + 1 */
+    int32_t n_isoforms;              /* 0 unless allele-specific */
+    int32_t n_parts;
+    const int32_t* isoform_start;    /* n_isoforms + 1, or NULL */
+    const int32_t* part_gene_start;  /* n_parts + 1: 0 ... n_genes */
+    int64_t n_samples;
+    int32_t threshold;
+    int32_t reserved;
+    uint64_t device_budget;
+} rsem_b200_ci_params;
+/* device time per phase, summed over the blocks (CUDA events) */
+typedef struct rsem_b200_ci_stats {
+    double transpose_ms;  /* sample-major -> transcript-major rows (with the column gather when not resident) */
+    double sums_ms;       /* FPKM rows, gene sums, isoform sums                                                 */
+    double sort_ms;       /* segmented sort of every row                                                        */
+    double interval_ms;   /* calcCI per row                                                                     */
+    uint64_t blocks;
+    int32_t resident;     /* 1: the sample matrix was kept on the device                                        */
+    int32_t reserved;
+} rsem_b200_ci_stats;
+/* allocates the sample matrix (Buffer.h:16-31 sizes a host buffer instead) */
+int rsem_b200_ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* params);
+/* count samples from index first: rows = count x M TPMs (tpm + 1 of calcCI.cpp:146), l_bars = count values.  Thread
+ * safe; the buffers may be reused when it returns (Buffer::write, Buffer.h:41-49)                                 */
+int rsem_b200_ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars, int64_t first, int64_t count);
+/* intervals as (lb, ub, cqv) of TPM then of FPKM, 6 floats per item: transcripts (M), genes (n_genes), isoforms
+ * (n_isoforms; may be NULL when 0) (calcCI.cpp:313-385, 446-496 prints them); frees the state                     */
+int rsem_b200_ci_end(rsem_b200_ctx* ctx, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats);
+
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);

@@ -1,7 +1,8 @@
 """In-tree build of every native artefact (called by __graft_entry__.build()).
 
   rsem_b200/librsem_b200.so   CUDA kernels + C ABI, sm_90a only
-  bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments, bin/rsem-simulate-reads
+  bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments, bin/rsem-simulate-reads,
+  bin/rsem-calculate-credibility-intervals
                               C++ drop-in executables (link the .so)
   tools/gen_dataset           synthetic intermediate-file generator (tooling)
   oracle/librsem_oracle.so    CPU restatement (test infrastructure)
@@ -49,8 +50,9 @@ def build_host(force: bool = False):
     common = sorted(glob.glob(os.path.join(HOST, "*.cpp")))
     mains = [s for s in common if os.path.basename(s).startswith("main_")]
     shared = [s for s in common if s not in mains]
-    # the simulator's tables are built in a file compiled with the reference's flags for simulation.cpp (-O3 -ffast-math,
-    # reference Makefile:39,72-73), so that they carry the same bits
+    # the simulator's tables and the credibility-interval sampler are built in files compiled with the reference's flags
+    # for simulation.cpp and calcCI.cpp (-O3 -ffast-math, reference Makefile:39,72-73), so that they carry the same bits;
+    # the link step adds no -ffast-math (no crtfastmath.o, which would set flush-to-zero for the whole process)
     ffm = sorted(glob.glob(os.path.join(HOST, "ffm", "*.cpp")))
     deps = common + ffm + glob.glob(os.path.join(HOST, "*.hpp")) + [os.path.join(ROOT, "include", "rsem_b200.h")]
     ffm_objs = []
@@ -62,9 +64,11 @@ def build_host(force: bool = False):
         ffm_objs.append(obj)
     for m in mains:
         name = {"main_em.cpp": "rsem-run-em", "main_gibbs.cpp": "rsem-run-gibbs", "main_simulate.cpp": "rsem-simulate-reads",
-                "main_selftest.cpp": "rsem-b200-host-selftest", "main_parse.cpp": "rsem-parse-alignments"}[os.path.basename(m)]
+                "main_selftest.cpp": "rsem-b200-host-selftest", "main_parse.cpp": "rsem-parse-alignments",
+                "main_ci.cpp": "rsem-calculate-credibility-intervals"}[os.path.basename(m)]
         out = os.path.join(ROOT, "bin", name)
-        extra = ffm_objs if name == "rsem-simulate-reads" else []
+        ffm_use = {"rsem-simulate-reads": "sim_tables.o", "rsem-calculate-credibility-intervals": "ci_sample.o"}
+        extra = [o for o in ffm_objs if os.path.basename(o) == ffm_use.get(name)]
         if force or _newer(out, deps + [os.path.join(ROOT, "rsem_b200", "librsem_b200.so")]):
             _run(["g++", "-O2", "-std=c++17", "-Wall", "-pthread", "-I", os.path.join(ROOT, "include"), "-o", out, m, *shared, *extra,
                   "-L", os.path.join(ROOT, "rsem_b200"), "-lrsem_b200", "-Wl,-rpath,$ORIGIN/../rsem_b200",
@@ -88,6 +92,7 @@ def build_oracle():
     # building the checker is not using it; `make ref` is a no-op when /root/reference is absent
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "all"])
     _run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "-f", "simulate.mk"])
+    _run(["make", "-s", "-C", os.path.join(ROOT, "oracle"), "-f", "ci.mk"])
 
 
 def build_all(force: bool = False):

@@ -69,6 +69,18 @@ class SimStats(C.Structure):
                 ("copy_ms", C.c_double), ("words", C.c_uint64), ("windows", C.c_uint64)]
 
 
+class CiParams(C.Structure):
+    _fields_ = [("M", C.c_int32), ("n_genes", C.c_int32), ("gene_start", C.POINTER(C.c_int32)),
+                ("n_isoforms", C.c_int32), ("n_parts", C.c_int32), ("isoform_start", C.POINTER(C.c_int32)),
+                ("part_gene_start", C.POINTER(C.c_int32)), ("n_samples", C.c_int64), ("threshold", C.c_int32),
+                ("reserved", C.c_int32), ("device_budget", C.c_uint64)]
+
+
+class CiStats(C.Structure):
+    _fields_ = [("transpose_ms", C.c_double), ("sums_ms", C.c_double), ("sort_ms", C.c_double),
+                ("interval_ms", C.c_double), ("blocks", C.c_uint64), ("resident", C.c_int32), ("reserved", C.c_int32)]
+
+
 def _dp(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
 
@@ -94,7 +106,7 @@ SYMBOLS = [
     "rsem_b200_gibbs_run", "rsem_b200_launch_count", "rsem_b200_estep_timing", "rsem_b200_set_profiling",
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
-    "rsem_b200_sim_end",
+    "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end",
 ]
 
 
@@ -304,6 +316,27 @@ class Context:
         stats = SimStats()
         self.lib.check(self.lib.dll.rsem_b200_sim_end(self._h, _dp(counts), C.byref(resim), C.byref(stats)))
         return counts, resim.value, stats
+
+    def ci_begin(self, params: CiParams):
+        """params' arrays must stay alive until ci_begin returns (they are copied)"""
+        self.lib.check(self.lib.dll.rsem_b200_ci_begin(self._h, C.byref(params)))
+
+    def ci_push(self, rows, l_bars, first: int):
+        """rows: count x M float32 TPMs of samples first .. first + count - 1, l_bars: their count mean lengths"""
+        rows, l_bars = _arr(rows, np.float32), _arr(l_bars, np.float32)
+        self.lib.check(self.lib.dll.rsem_b200_ci_push(self._h, _p(rows, C.c_float), _p(l_bars, C.c_float),
+                                                      C.c_int64(first), C.c_int64(len(l_bars))))
+
+    def ci_end(self, M: int, n_genes: int, n_isoforms: int = 0):
+        """-> (transcripts M x 6, genes n_genes x 6, isoforms n_isoforms x 6, CiStats); columns are the TPM lb, ub, cqv
+        and the FPKM lb, ub, cqv"""
+        tr = np.zeros((M, 6), np.float32)
+        ge = np.zeros((n_genes, 6), np.float32)
+        iso = np.zeros((n_isoforms, 6), np.float32)
+        stats = CiStats()
+        self.lib.check(self.lib.dll.rsem_b200_ci_end(self._h, _p(tr, C.c_float), _p(ge, C.c_float),
+                                                     _p(iso, C.c_float) if n_isoforms else None, C.byref(stats)))
+        return tr, ge, iso, stats
 
     # ---- instrumentation
     def launch_count(self) -> int:

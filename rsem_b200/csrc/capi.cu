@@ -287,6 +287,7 @@ int rsem_b200_ctx_destroy(rsem_b200_ctx* c) {
     free_refs(c);
     free_gibbs(c);
     sim_free(c);
+    ci_free(c);
     if (c->model_buf) cudaFree(c->model_buf);
     if (c->stats_buf) cudaFree(c->stats_buf);
     if (c->d_stats) cudaFree(c->d_stats);
@@ -748,6 +749,36 @@ int rsem_b200_sim_end(rsem_b200_ctx* c, double* counts, uint64_t* resim, rsem_b2
     RB_ARG(c, "NULL argument");
     RB_CUDA(cudaSetDevice(c->device));
     return sim_end(c, counts, resim, stats);
+}
+
+int rsem_b200_ci_begin(rsem_b200_ctx* c, const rsem_b200_ci_params* p) {
+    RB_ARG(c && p, "NULL argument");
+    RB_ARG(p->M >= 1 && p->n_genes >= 1 && p->n_samples >= 1 && p->n_parts >= 1, "bad M, gene count, sample count or parts");
+    RB_ARG(p->gene_start && p->part_gene_start && (p->n_isoforms == 0 || p->isoform_start), "NULL group array");
+    RB_ARG(p->gene_start[0] == 1 && p->gene_start[p->n_genes] == p->M + 1, "gene_start must cover transcripts 1..M");
+    for (int32_t g = 0; g < p->n_genes; ++g) RB_ARG(p->gene_start[g] < p->gene_start[g + 1], "empty gene");
+    RB_ARG(p->part_gene_start[0] == 0 && p->part_gene_start[p->n_parts] == p->n_genes, "parts must cover the genes");
+    for (int32_t i = 0; i < p->n_parts; ++i) RB_ARG(p->part_gene_start[i] <= p->part_gene_start[i + 1], "parts out of order");
+    if (p->n_isoforms) {
+        RB_ARG(p->isoform_start[0] == 1 && p->isoform_start[p->n_isoforms] == p->M + 1, "isoform_start must cover 1..M");
+        for (int32_t i = 0; i < p->n_isoforms; ++i) RB_ARG(p->isoform_start[i] < p->isoform_start[i + 1], "empty isoform");
+    }
+    RB_ARG(p->n_samples <= INT32_MAX, "too many samples");
+    RB_CUDA(cudaSetDevice(c->device));
+    return ci_begin(c, p);
+}
+
+int rsem_b200_ci_push(rsem_b200_ctx* c, const float* rows, const float* l_bars, int64_t first, int64_t count) {
+    RB_ARG(c && (count == 0 || (rows && l_bars)), "NULL argument");
+    RB_CUDA(cudaSetDevice(c->device));
+    return ci_push(c, rows, l_bars, first, count);
+}
+
+int rsem_b200_ci_end(rsem_b200_ctx* c, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats) {
+    RB_ARG(c && transcripts && genes, "NULL argument");
+    RB_ARG(c->ci, "ci_begin must be called first");
+    RB_CUDA(cudaSetDevice(c->device));
+    return ci_end(c, transcripts, genes, isoforms, stats);
 }
 
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {

@@ -149,6 +149,7 @@ struct ClassLayout {
 };
 
 struct SimState;  // sim_kernels.cu
+struct CiState;   // ci_kernels.cu
 
 }  // namespace rsem_b200
 
@@ -223,6 +224,7 @@ struct rsem_b200_ctx {
 
     rsem_b200::DevGibbs gibbs;
     rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads between sim_begin and sim_end
+    rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals between ci_begin and ci_end
 
     // multi-GPU
     void* comm = nullptr;
@@ -307,5 +309,11 @@ int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p);
 int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
 int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 void sim_free(rsem_b200_ctx* ctx);
+
+// ci_kernels.cu
+int ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* p);
+int ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars, int64_t first, int64_t count);
+int ci_end(rsem_b200_ctx* ctx, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats);
+void ci_free(rsem_b200_ctx* ctx);
 
 }  // namespace rsem_b200

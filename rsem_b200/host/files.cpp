@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
+#include <set>
 #include <thread>
 
 #include "host.hpp"
@@ -52,6 +53,19 @@ std::vector<char> slurp(const std::string& path, bool must_exist) {
     }
     fclose(f);
     return buf;
+}
+
+std::vector<uint32_t> engine_seeds(uint32_t seed, int n) {
+    Mt seedEngine(seed);
+    std::set<uint32_t> used;
+    std::vector<uint32_t> out(n);
+    for (int i = 0; i < n; ++i) {
+        uint32_t s;
+        do { s = seedEngine.next(); } while (used.count(s));
+        used.insert(s);
+        out[i] = s;
+    }
+    return out;
 }
 
 uint32_t parse_seed(const char* s) {

@@ -283,6 +283,8 @@ struct Mt {
 };
 
 // ---- small utilities -----------------------------------------------------------------------------
+// engineFactory (sampling.h:19-40): n engine seeds drawn from mt19937(seed), a seed already handed out is skipped
+std::vector<uint32_t> engine_seeds(uint32_t seed, int n);
 std::vector<char> slurp(const std::string& path, bool must_exist = true);
 void read_type_files(const std::string& imd_name, int tag, int read_type, std::vector<std::string>& files);
 uint32_t parse_seed(const char* s);  // digit-by-digit as EM.cpp:588-593

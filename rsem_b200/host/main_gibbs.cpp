@@ -12,7 +12,6 @@
 #include <chrono>
 #include <ctime>
 #include <future>
-#include <set>
 #include <thread>
 
 #include "host.hpp"
@@ -144,18 +143,10 @@ int main(int argc, char* argv[]) {
 
     // init(): samples per chain and per-chain engines (Gibbs.cpp:207-254)
     std::vector<int32_t> chain_samples(nThreads);
-    std::vector<uint32_t> chain_seeds(nThreads);
+    std::vector<uint32_t> chain_seeds = engine_seeds(hasSeed ? seed : (uint32_t)time(NULL), nThreads);
     {
         const int quotient = NSAMPLES / nThreads, left = NSAMPLES % nThreads;
-        Mt seedEngine(hasSeed ? seed : (uint32_t)time(NULL));
-        std::set<uint32_t> used;
-        for (int i = 0; i < nThreads; ++i) {
-            chain_samples[i] = quotient + (i < left ? 1 : 0);
-            uint32_t s;
-            do { s = seedEngine.next(); } while (used.count(s));
-            used.insert(s);
-            chain_seeds[i] = s;
-        }
+        for (int i = 0; i < nThreads; ++i) chain_samples[i] = quotient + (i < left ? 1 : 0);
     }
     if (g_verbose) printf("Initialization finished!\n");
 
