@@ -313,7 +313,8 @@ __device__ double conprb_single(const ModelArgs& a, const double* prof, unsigned
         for (int fragLen = minL; fragLen <= maxL; ++fragLen) {
             const int pfpos = dir == 0 ? pos : totLen - pos - fragLen;
             const int effL = min(fullLen, totLen - fragLen + 1);
-            value += ld_adj(m.gld, fragLen, totLen) * rspd_adj(m, pfpos, effL, fullLen) * ld_adj(m.mld, readLen, fragLen);
+            // __dadd_rn: a separate rounded add, as in the reference's loop (nvcc would otherwise contract it into an FMA)
+            value = __dadd_rn(value, ld_adj(m.gld, fragLen, totLen) * rspd_adj(m, pfpos, effL, fullLen) * ld_adj(m.mld, readLen, fragLen));
         }
     } else {
         const int effL = min(fullLen, totLen - readLen + 1);
@@ -1031,7 +1032,7 @@ int launch_update_g(rsem_b200_ctx* c, ModelArgs& a, unsigned grid) {
         if (rc) return rc;
         a.mode = 2;
     }
-    static const bool global_reds = getenv("RSEM_B200_K3") && !strcmp(getenv("RSEM_B200_K3"), "global");
+    const bool global_reds = getenv("RSEM_B200_K3") && !strcmp(getenv("RSEM_B200_K3"), "global");
     if (hasq && !global_reds) return paired ? launch_update_q<G, true>(c, a) : launch_update_q<G, false>(c, a);
     if (hasq && paired) update_kernel<G, true, true><<<grid, kBlock, 0, c->stream>>>(a);
     else if (hasq) update_kernel<G, true, false><<<grid, kBlock, 0, c->stream>>>(a);
@@ -1091,7 +1092,7 @@ int model_launch_conprb(rsem_b200_ctx* c) {
     if (c->N == 0) return 0;
     // reads whose hits all show them the same bases take the cooperative path (one pass over the bases per READ instead
     // of per hit); RSEM_B200_NO_COOP=1 keeps every read on the per-hit path (the reference's multiplication order)
-    static const bool no_coop = getenv("RSEM_B200_NO_COOP") != nullptr;
+    const bool no_coop = getenv("RSEM_B200_NO_COOP") != nullptr;
     if (!no_coop) if (int rc = ensure_uniform_flags(c)) return rc;
     ModelArgs a;
     fill_args(c, a);

@@ -47,6 +47,14 @@ class Oracle:
                           _p(post, C.c_double), _p(post0, C.c_double), C.c_int32(n_threads))
         return (counts, post, post0) if want_post else counts
 
+    def mstep(self, counts, theta, n0):
+        """-> (new theta, (sum, bchange, totnum)); theta is the one the round started from"""
+        counts, theta = c64(counts).copy(), c64(theta).copy()
+        st = RoundStats()
+        self.dll.ro_mstep(C.c_int32(len(theta) - 1), _p(counts, C.c_double), _p(theta, C.c_double), C.c_double(n0),
+                          C.byref(st))
+        return theta, (st.sum, st.bchange, st.totnum)
+
     def em_rounds(self, row_ptr, sid, conprb, ncpv, theta, n0, first_round, max_rounds, min_round, max_round, n_threads=1):
         row_ptr = np.ascontiguousarray(row_ptr, np.uint64); sid = np.ascontiguousarray(sid, np.int32)
         conprb, ncpv = c64(conprb), c64(ncpv)
