@@ -326,6 +326,41 @@ int rsem_b200_ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars
  * (n_isoforms; may be NULL when 0) (calcCI.cpp:313-385, 446-496 prints them); frees the state                     */
 int rsem_b200_ci_end(rsem_b200_ctx* ctx, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats);
 
+/* ---- rsem-for-ebseq-calculate-clustering-info (K9, kmer_kernels.cu) ----------------------------------------------------
+ * Replaces the k-mer candidate list, its std::sort and the pass over groups of equal k-mers
+ * (EBSeq/calcClusteringInfo.cpp:101-130).  Transcript t (0-based, input order) is bases[offsets[t] .. offsets[t + 1]), one
+ * code per base: 0 A, 1 C, 2 G, 3 T, 4 N (the caller maps every other letter to N, as convert() does, :51-59).  For each
+ * t, shared_counts[t] = the number of start positions j in [0, len_t - k + 1) whose k-mer (forward strand) also starts at
+ * some position of a different transcript: the sum of the group runs with numerator < denominator (:117-130).  Repeats
+ * inside one transcript do not count; N matches N.  The ratio the tool prints is shared_counts[t] / effL_t (:132-134).
+ * max_device_bytes: device memory for the packed bases, the offsets, the counts and the hash table (0 = what is free
+ * less 512 MB).  When a table of 2 slots (12 bytes each) per position does not fit, the k-mers are split by hash into
+ * passes = ceil(2 positions / table slots) passes over one table; the counts are the same for every budget.
+ * fingerprint_bits: bits of the hash kept in a slot beside the position (0 = 24; 1..24).  Equal fingerprints are
+ * verified base by base, so the counts do not depend on it; small values make most probes verify (tests).          */
+typedef struct rsem_b200_kmer_params {
+    int32_t k;                   /* >= 1 */
+    int32_t fingerprint_bits;
+    uint64_t n_transcripts;
+    const uint64_t* offsets;     /* n_transcripts + 1, offsets[0] = 0, non-decreasing */
+    const uint8_t* bases;        /* offsets[n_transcripts] codes 0..4 */
+    uint64_t max_device_bytes;
+} rsem_b200_kmer_params;
+/* device time per phase (CUDA events), summed over the passes */
+typedef struct rsem_b200_kmer_stats {
+    uint64_t positions;     /* k-mer start positions (the reference's cands.size()) */
+    uint64_t table_slots;
+    uint64_t input_bytes;   /* packed bases (2 + 1 bits per base), offsets and counts */
+    uint64_t table_bytes;
+    int32_t passes;         /* 0 when there are no positions (no device work) */
+    int32_t reserved;
+    double pack_ms;         /* bases to the device and packing */
+    double insert_ms;       /* table clearing and the insert pass */
+    double count_ms;        /* the count pass */
+} rsem_b200_kmer_stats;
+int rsem_b200_kmer_shared(rsem_b200_ctx* ctx, const rsem_b200_kmer_params* params, uint64_t* shared_counts,
+                          rsem_b200_kmer_stats* stats /* may be NULL */);
+
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);

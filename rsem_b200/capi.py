@@ -81,6 +81,17 @@ class CiStats(C.Structure):
                 ("interval_ms", C.c_double), ("blocks", C.c_uint64), ("resident", C.c_int32), ("reserved", C.c_int32)]
 
 
+class KmerParams(C.Structure):
+    _fields_ = [("k", C.c_int32), ("fingerprint_bits", C.c_int32), ("n_transcripts", C.c_uint64),
+                ("offsets", C.POINTER(C.c_uint64)), ("bases", C.POINTER(C.c_uint8)), ("max_device_bytes", C.c_uint64)]
+
+
+class KmerStats(C.Structure):
+    _fields_ = [("positions", C.c_uint64), ("table_slots", C.c_uint64), ("input_bytes", C.c_uint64),
+                ("table_bytes", C.c_uint64), ("passes", C.c_int32), ("reserved", C.c_int32), ("pack_ms", C.c_double),
+                ("insert_ms", C.c_double), ("count_ms", C.c_double)]
+
+
 def _dp(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
 
@@ -106,7 +117,7 @@ SYMBOLS = [
     "rsem_b200_gibbs_run", "rsem_b200_launch_count", "rsem_b200_estep_timing", "rsem_b200_set_profiling",
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
-    "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end",
+    "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end", "rsem_b200_kmer_shared",
 ]
 
 
@@ -337,6 +348,19 @@ class Context:
         self.lib.check(self.lib.dll.rsem_b200_ci_end(self._h, _p(tr, C.c_float), _p(ge, C.c_float),
                                                      _p(iso, C.c_float) if n_isoforms else None, C.byref(stats)))
         return tr, ge, iso, stats
+
+    def kmer_shared(self, k: int, offsets, bases, max_device_bytes: int = 0, fingerprint_bits: int = 0):
+        """-> (per transcript, the start positions whose k-mer also starts in another transcript, uint64; KmerStats).
+        offsets: n + 1 transcript offsets into bases, codes 0..4 (A C G T N)"""
+        offsets, bases = _arr(offsets, np.uint64), _arr(bases, np.uint8)
+        n = len(offsets) - 1
+        counts = np.zeros(max(n, 1), np.uint64)
+        params = KmerParams(k=k, fingerprint_bits=fingerprint_bits, n_transcripts=n, offsets=_p(offsets, C.c_uint64),
+                            bases=_p(bases, C.c_uint8), max_device_bytes=max_device_bytes)
+        stats = KmerStats()
+        self.lib.check(self.lib.dll.rsem_b200_kmer_shared(self._h, C.byref(params), _p(counts, C.c_uint64),
+                                                          C.byref(stats)))
+        return counts[:n], stats
 
     # ---- instrumentation
     def launch_count(self) -> int:

@@ -781,6 +781,19 @@ int rsem_b200_ci_end(rsem_b200_ctx* c, float* transcripts, float* genes, float* 
     return ci_end(c, transcripts, genes, isoforms, stats);
 }
 
+int rsem_b200_kmer_shared(rsem_b200_ctx* c, const rsem_b200_kmer_params* p, uint64_t* shared_counts,
+                          rsem_b200_kmer_stats* stats) {
+    RB_ARG(c && p && p->offsets && (shared_counts || p->n_transcripts == 0), "NULL argument");
+    RB_ARG(p->k >= 1, "k must be >= 1");
+    RB_ARG(p->fingerprint_bits >= 0 && p->fingerprint_bits <= 24, "fingerprint_bits must be 0..24");
+    RB_ARG(p->offsets[0] == 0, "offsets[0] must be 0");
+    for (uint64_t t = 0; t < p->n_transcripts; ++t) RB_ARG(p->offsets[t] <= p->offsets[t + 1], "offsets must not decrease");
+    RB_ARG(p->bases || p->offsets[p->n_transcripts] == 0, "NULL bases");
+    RB_ARG(p->n_transcripts < 0xffffffffull, "too many transcripts");
+    RB_CUDA(cudaSetDevice(c->device));
+    return kmer_shared(c, p, shared_counts, stats);
+}
+
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {
     RB_ARG(c && launches, "NULL argument");
     *launches = c->launches;

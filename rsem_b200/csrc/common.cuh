@@ -316,4 +316,7 @@ int ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars, int64_t 
 int ci_end(rsem_b200_ctx* ctx, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats);
 void ci_free(rsem_b200_ctx* ctx);
 
+// kmer_kernels.cu
+int kmer_shared(rsem_b200_ctx* ctx, const rsem_b200_kmer_params* p, uint64_t* counts, rsem_b200_kmer_stats* stats);
+
 }  // namespace rsem_b200
