@@ -370,9 +370,9 @@ int rsem_b200_estep_timing(rsem_b200_ctx* ctx, double* total_ms, uint64_t* launc
 /* enable per-launch event timing of K2 (off by default: it adds two event records per round)    */
 int rsem_b200_set_profiling(rsem_b200_ctx* ctx, int32_t enabled);
 /* select the E/M kernel variant: 0 = auto (equivalence-class layout for frozen-conprb rounds, row groups when
- * posteriors are written), 1 = CTA-staged tiles (TMA), 2 = direct (no smem staging), 3 = warp-pipelined tiles
- * (TMA, no CTA barriers), 4 = row groups on CTA-staged tiles (TMA, no CTA barriers, dynamic row batches),
- * 5 = equivalence-class layout, fail if the matrix is outside its limits                           */
+ * posteriors are written), 2 = direct (no smem staging), 4 = row groups on CTA-staged tiles (TMA, no CTA
+ * barriers, dynamic row batches), 5 = equivalence-class layout, fail if the matrix is outside its limits.
+ * Any other value returns RSEM_B200_ERR_ARG.                                                          */
 int rsem_b200_set_estep_variant(rsem_b200_ctx* ctx, int32_t variant);
 
 /* Equivalence-class layout the frozen-conprb rounds run on (derived from the hit matrix on first use; reads with

@@ -89,15 +89,11 @@ void free_hits(rsem_b200_ctx* c) {
     dev_free(c, &c->ncpv, c->N);
     if (c->post) dev_free(c, &c->post, c->H);
     if (c->post0) dev_free(c, &c->post0, c->N);
-    if (c->theta_tex) { cudaDestroyTextureObject(c->theta_tex); c->theta_tex = 0; c->theta_tex_ptr = nullptr; }
     if (c->theta) dev_free(c, &c->theta, (size_t)c->M + 1);
     if (c->count) dev_free(c, &c->count, (size_t)c->M + 1);
     if (c->tile_row) { cudaFree(c->tile_row); c->tile_row = nullptr; }   // small (16 B per ~4000 hits)
     if (c->tile_hit) { cudaFree(c->tile_hit); c->tile_hit = nullptr; }
-    if (c->tile_meta) { cudaFree(c->tile_meta); c->tile_meta = nullptr; }
-    if (c->wtile_row) { cudaFree(c->wtile_row); c->wtile_row = nullptr; }
-    if (c->wtile_hit) { cudaFree(c->wtile_hit); c->wtile_hit = nullptr; }
-    c->n_tiles = c->n_wtiles = 0;
+    c->n_tiles = 0;
     class_free(c);
     if (c->reads.uni) { cudaFree(c->reads.uni); c->reads.uni = nullptr; }   // sized by N, derived from the hits
     c->reads.uni_valid = false;
@@ -856,7 +852,8 @@ int rsem_b200_estep_wait_times(rsem_b200_ctx* c, uint64_t* out_ns, int32_t cap, 
 }
 
 int rsem_b200_set_estep_variant(rsem_b200_ctx* c, int32_t v) {
-    RB_ARG(c && v >= 0 && v <= 5, "variant must be 0..5");
+    RB_ARG(c && (v == 0 || v == 2 || v == 4 || v == 5),
+           "variant must be 0 (auto), 2 (direct), 4 (row groups on staged tiles) or 5 (class layout)");
     c->variant = v;
     return 0;
 }

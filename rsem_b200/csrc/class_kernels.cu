@@ -31,6 +31,7 @@
 #include <ctime>
 
 #include "common.cuh"
+#include "tma.cuh"
 
 namespace rsem_b200 {
 
@@ -73,27 +74,7 @@ struct TileRec {
     unsigned long long val_begin, id_begin, batch_begin;
 };
 
-// ---- PTX helpers (same idioms as em_kernels.cu) ------------------------------------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "CW_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra CW_DONE;\n"
-        "bra CW_WAIT;\n"
-        "CW_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
+// ---- PTX helpers beyond tma.cuh ----------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
@@ -109,18 +90,6 @@ __device__ __forceinline__ void mbar_wait_timed(unsigned long long* bar, unsigne
         mbar_wait(bar, parity);
     }
 }
-__device__ __forceinline__ void bulk_load(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void red_add_f64(double* addr, double v) {
-    asm volatile("red.global.add.f64 [%0], %1;" ::"l"(addr), "d"(v) : "memory");
-}
-__device__ __forceinline__ unsigned round16(unsigned bytes) { return (bytes + 15u) & ~15u; }
 
 // ------------------------------------------------------------------------------------------------------------------
 // directory construction

@@ -189,22 +189,13 @@ struct rsem_b200_ctx {
     // E-step tiling (em_kernels.cu)
     uint64_t* tile_row = nullptr;
     uint64_t* tile_hit = nullptr;
-    void* tile_meta = nullptr;      // per-tile head masks (em_kernels.cu TileMeta)
     uint32_t n_tiles = 0;
-    uint64_t* wtile_row = nullptr;  // warp-pipelined kernel's own (smaller) tiles
-    uint64_t* wtile_hit = nullptr;
-    uint32_t n_wtiles = 0;
     int group = 16;       // lanes cooperating on one row (K1 / K3 / direct K2)
-    int tma_group = 4;    // lanes per row in phase B of the staged K2
     int rows_group = 8;   // lanes per row of the row-group K2 (variant 4)
-    bool tiles_for_rows = true;  // tiles built for the row-group kernel (no row-start masks) or for the three-phase one
-    int cta_threads = 512;  // threads per CTA of the staged K2 (tile geometry depends on it)
-    int variant = 0;      // 0 auto, 1 CTA-staged, 2 direct, 3 warp-pipelined, 4 row groups, 5 class layout
+    int variant = 0;      // 0 auto, 2 direct, 4 row groups, 5 class layout
 
     // EM state
     double* theta = nullptr;   // M + 1
-    cudaTextureObject_t theta_tex = 0;  // optional texture view of theta (em_kernels.cu)
-    const double* theta_tex_ptr = nullptr;
     double* count = nullptr;   // M + 1
     int* done_flag = nullptr;  // device int: 1 once the loop condition ended the run
     int* err_flag = nullptr;
@@ -261,7 +252,7 @@ int dev_alloc(rsem_b200_ctx* ctx, T** p, size_t n) {
     void* q = nullptr;
     cudaError_t e = block_alloc(ctx, &q, bytes);
     if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc", __FILE__, __LINE__);
-    // the padding is read (never used) by the pair-wise phases of the staged E-step: keep it defined
+    // the padding is read (never used) by the E-step's bulk copies, which round up to 16 B: keep it defined
     cudaMemset(static_cast<char*>(q) + n * sizeof(T), 0, 256);
     ctx->dev_bytes += bytes;
     *p = static_cast<T*>(q);
