@@ -361,6 +361,54 @@ typedef struct rsem_b200_kmer_stats {
 int rsem_b200_kmer_shared(rsem_b200_ctx* ctx, const rsem_b200_kmer_params* params, uint64_t* shared_counts,
                           rsem_b200_kmer_stats* stats /* may be NULL */);
 
+/* ---- rsem-tbam2gbam (K10, gbam_kernels.cu) -----------------------------------------------------------------------------
+ * Replaces the per-alignment work of BamConverter::process (BamConverter.h:92-303): convert() with tr2chr
+ * (sam_utils.h:137-208), flipSeq / flipQual, modifyTags, the CollapseMap of each read (bc_aux.h) and
+ * writeCollapsedLines.  One call converts one batch of whole groups and returns the output records in output order.
+ *
+ * Batch: every record as BAM stores it, preceded by its u32 block_size, at data + rec_off[r].  A unit is one record or
+ * a mate pair (mate 1 first): records [unit_rec[u], unit_rec[u + 1]).  unit_tr[u] = the transcript (1..M) of a mapped
+ * unit, 0 for an unmapped unit, which is written through unchanged.  unit_group[u] is non-decreasing; the mapped units
+ * of one group (a run of one read name) collapse as in CollapseMap; an unmapped unit is a group of its own.
+ * The caller does the framing and the validation the reference does while it reads (BamConverter.h:110-150).
+ *
+ * Tables (uploaded on the first call with a given `tables` pointer and kept until the context is destroyed):
+ * out_tid[t] = the chrlist index of transcript t's seqname (-1: not in the chrlist); minus[t] = 1 on '-' strand;
+ * exons of t are [exon_off[t], exon_off[t + 1]) as 1-based inclusive (start, end), ascending (Transcript.h:119-148).
+ * mapq_prb[m] = the smallest float prb >= 0 with bam_prb_to_mapq(prb) >= m, m = 1..100 (sam_utils.h:72-76, built on
+ * the host with the host's log10); the device gives MAPQ = #{m : prb >= mapq_prb[m]}.
+ *
+ * out: out_cap bytes; *out_bytes = what the batch wrote (block_size + record, in output order).  On a record the
+ * reference would abort on (a base code other than 1/2/4/8/15, a negative genomic position, a read outside the exons,
+ * a transcript without a chrlist entry, a kept pair whose mate 2 lacks the ZW of mate 1, a ZW sum below 0 or NaN,
+ * an optional field of unknown type) the call returns RSEM_B200_ERR_ARG with stats->bad_unit = the first such unit. */
+typedef struct rsem_b200_gbam_tables {
+    int32_t M;
+    int32_t reserved;
+    const int32_t* out_tid;     /* M + 1 */
+    const uint8_t* minus;       /* M + 1 */
+    const int32_t* length;      /* M + 1: Transcript::length */
+    const int64_t* exon_off;    /* M + 2 */
+    const int32_t* exon_start;  /* exon_off[M + 1] */
+    const int32_t* exon_end;
+    const float* mapq_prb;      /* 101; [0] unused */
+} rsem_b200_gbam_tables;
+typedef struct rsem_b200_gbam_batch {
+    uint64_t n_records, n_units, n_bytes;
+    const uint8_t* data;        /* n_bytes */
+    const uint64_t* rec_off;    /* n_records */
+    const uint32_t* unit_rec;   /* n_units + 1 */
+    const uint32_t* unit_group; /* n_units */
+    const int32_t* unit_tr;     /* n_units */
+} rsem_b200_gbam_batch;
+typedef struct rsem_b200_gbam_stats {
+    double device_ms;           /* CUDA events: copies in, convert, sort, collapse, emit, copy out */
+    uint64_t units_written;     /* kept + written-through units */
+    int64_t bad_unit;           /* -1 unless the call failed on a record */
+} rsem_b200_gbam_stats;
+int rsem_b200_gbam_convert(rsem_b200_ctx* ctx, const rsem_b200_gbam_tables* tables, const rsem_b200_gbam_batch* batch,
+                           uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, rsem_b200_gbam_stats* stats /* may be NULL */);
+
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);

@@ -118,6 +118,7 @@ SYMBOLS = [
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
     "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end", "rsem_b200_kmer_shared",
+    "rsem_b200_gbam_convert",
 ]
 
 

@@ -284,6 +284,7 @@ int rsem_b200_ctx_destroy(rsem_b200_ctx* c) {
     free_gibbs(c);
     sim_free(c);
     ci_free(c);
+    gbam_free(c);
     if (c->model_buf) cudaFree(c->model_buf);
     if (c->stats_buf) cudaFree(c->stats_buf);
     if (c->d_stats) cudaFree(c->d_stats);
@@ -788,6 +789,18 @@ int rsem_b200_kmer_shared(rsem_b200_ctx* c, const rsem_b200_kmer_params* p, uint
     RB_ARG(p->n_transcripts < 0xffffffffull, "too many transcripts");
     RB_CUDA(cudaSetDevice(c->device));
     return kmer_shared(c, p, shared_counts, stats);
+}
+
+int rsem_b200_gbam_convert(rsem_b200_ctx* c, const rsem_b200_gbam_tables* t, const rsem_b200_gbam_batch* b, uint8_t* out,
+                           uint64_t out_cap, uint64_t* out_bytes, rsem_b200_gbam_stats* stats) {
+    RB_ARG(c && t && b && out_bytes && (out || out_cap == 0), "NULL argument");
+    RB_ARG(t->M >= 1 && t->out_tid && t->minus && t->length && t->exon_off && t->mapq_prb, "NULL or empty transcript table");
+    RB_ARG(t->exon_off[0] == 0 && (t->exon_off[t->M + 1] == 0 || (t->exon_start && t->exon_end)), "bad exon table");
+    RB_ARG(b->n_units == 0 || (b->data && b->rec_off && b->unit_rec && b->unit_group && b->unit_tr), "NULL batch array");
+    RB_ARG(b->n_units < 0xffffffffull && b->n_records < 0xffffffffull, "batch too large");
+    RB_ARG(b->n_units == 0 || (b->unit_rec[0] == 0 && b->unit_rec[b->n_units] == b->n_records), "unit_rec must cover the records");
+    RB_CUDA(cudaSetDevice(c->device));
+    return gbam_convert(c, t, b, out, out_cap, out_bytes, stats);
 }
 
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {

@@ -150,6 +150,7 @@ struct ClassLayout {
 
 struct SimState;  // sim_kernels.cu
 struct CiState;   // ci_kernels.cu
+struct GbamState; // gbam_kernels.cu
 
 }  // namespace rsem_b200
 
@@ -216,6 +217,7 @@ struct rsem_b200_ctx {
     rsem_b200::DevGibbs gibbs;
     rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads between sim_begin and sim_end
     rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals between ci_begin and ci_end
+    rsem_b200::GbamState* gbam = nullptr;  // rsem-tbam2gbam: transcript tables and batch scratch
 
     // multi-GPU
     void* comm = nullptr;
@@ -309,5 +311,10 @@ void ci_free(rsem_b200_ctx* ctx);
 
 // kmer_kernels.cu
 int kmer_shared(rsem_b200_ctx* ctx, const rsem_b200_kmer_params* p, uint64_t* counts, rsem_b200_kmer_stats* stats);
+
+// gbam_kernels.cu
+int gbam_convert(rsem_b200_ctx* ctx, const rsem_b200_gbam_tables* t, const rsem_b200_gbam_batch* b, uint8_t* out,
+                 uint64_t out_cap, uint64_t* out_bytes, rsem_b200_gbam_stats* stats);
+void gbam_free(rsem_b200_ctx* ctx);
 
 }  // namespace rsem_b200

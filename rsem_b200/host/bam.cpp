@@ -704,10 +704,30 @@ bool BamRecord::aux_int(const char tag[2], long long& value) const {
 }
 
 // MAPQ + ZW:f from the posterior (BamWriter.h:39-48, sam_utils.h:72-76)
-void BamRecord::set_alignment_weight(double prb) {
+uint8_t prb_to_mapq(double prb) {
     const double err = 1.0 - prb;
-    const uint8_t mapq = err <= 1e-10 ? 100 : (uint8_t)(-10 * std::log10(err) + .5);
-    data[9] = mapq;  // bin_mq_nl: byte 8 = l_read_name, byte 9 = MAPQ
+    return err <= 1e-10 ? 100 : (uint8_t)(-10 * std::log10(err) + .5);
+}
+
+std::vector<float> mapq_thresholds() {
+    std::vector<float> t(101, 0.0f);
+    const uint32_t hi = 0x40000000u;   // 2.0f; every p >= 1 gives 100
+    for (int m = 1; m <= 100; ++m) {   // bisection over the ordered bit patterns of the non-negative floats
+        uint32_t lo = 0, up = hi;
+        while (lo < up) {
+            const uint32_t mid = lo + (up - lo) / 2;
+            float p;
+            memcpy(&p, &mid, 4);
+            if (prb_to_mapq(p) >= m) up = mid;
+            else lo = mid + 1;
+        }
+        memcpy(&t[m], &lo, 4);
+    }
+    return t;
+}
+
+void BamRecord::set_alignment_weight(double prb) {
+    data[9] = prb_to_mapq(prb);  // bin_mq_nl: byte 8 = l_read_name, byte 9 = MAPQ
     const float val = (float)prb;
     // walk the optional fields to find an existing ZW
     const uint32_t l_name = data[8], n_cig = rd_u32(data.data() + 12) & 0xffff;
@@ -740,7 +760,8 @@ void BamRecord::set_alignment_weight(double prb) {
 }
 
 // ---- header text as the reference rewrites it (SamHeader.cpp:74-114 + insertPG, SamHeader.hpp:38-60) -------------------
-std::string rsem_bam_header_text(const std::string& in_text) {
+std::string rsem_bam_header_text(const std::string& in_text, const std::string& pg_id, const std::string& pg_cl,
+                                 const std::string* sq, bool reference_pg_ids) {
     std::string HD, SQ, RG, PG, CO, other;
     std::vector<std::string> pids;
     size_t fr = 0;
@@ -758,19 +779,26 @@ std::string rsem_bam_header_text(const std::string& in_text) {
         else if (tag == "RG") RG += line + "\n";
         else if (tag == "PG") {
             std::string id;
+            bool has_id = false;
             for (size_t a = 4; a < line.size();) {
                 size_t b = line.find('\t', a);
-                if (b == std::string::npos) b = line.size();
-                if (line.compare(a, 3, "ID:") == 0) id = line.substr(a + 3, b - a - 3);
+                if (line.compare(a, 3, "ID:") == 0) {
+                    // SamHeader::parse_line takes line.substr(fr, to) with `to` an index
+                    id = reference_pg_ids ? line.substr(a, b).substr(3) : line.substr(a + 3, (b == std::string::npos ? line.size() : b) - a - 3);
+                    has_id = true;
+                }
+                if (b == std::string::npos) break;
                 a = b + 1;
             }
+            if (reference_pg_ids && !has_id) die("\"" + line + "\" does not contain an ID!");
             if (std::find(pids.begin(), pids.end(), id) != pids.end()) die("Program record identifier " + id + " is not unique!");
             pids.push_back(id);
             PG += line + "\n";
         } else if (tag == "CO") CO += line + "\n";
         else other += line;  // sic: the reference appends these lines without their newline (SamHeader.cpp:111)
     }
-    if (std::find(pids.begin(), pids.end(), std::string("RSEM")) == pids.end()) PG += "@PG\tID:RSEM\n";
+    if (sq) SQ = *sq;
+    if (std::find(pids.begin(), pids.end(), pg_id) == pids.end()) PG += "@PG\tID:" + pg_id + (pg_cl.empty() ? "" : "\tCL:" + pg_cl) + "\n";
     return HD + SQ + RG + PG + CO + other;
 }
 
@@ -841,6 +869,8 @@ void BamWriter::append(const uint8_t* p, size_t n) {
     pending_.insert(pending_.end(), p, p + n);
     if (pending_.size() >= kBgzfBlock * 64 * (size_t)threads_) flush_pending(false);
 }
+
+void BamWriter::write_encoded(const uint8_t* p, size_t n) { append(p, n); }
 
 void BamWriter::write(const BamRecord& rec) {
     uint8_t b4[4];

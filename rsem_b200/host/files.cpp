@@ -205,10 +205,38 @@ void load_transcripts(const std::string& path, std::vector<TranscriptInfo>& out,
         std::string strand;
         int s;
         fin >> strand >> t.length >> s;
-        for (int k = 0; k < s; ++k) { int a, b; fin >> a >> b; }
+        t.strand = strand.empty() ? '+' : strand[0];
+        for (int k = 0; k < s; ++k) {
+            int a, b;
+            fin >> a >> b;
+            t.exons.emplace_back(a, b);
+            t.exon_length += b - a + 1;
+        }
         getline(fin, line);
         getline(fin, line);  // "left"
     }
+}
+
+std::vector<int> map_bam_targets(const std::vector<std::string>& names, const std::vector<TranscriptInfo>& tr, int ti_type) {
+    const int M = (int)tr.size() - 1;
+    if (names.empty()) die("The SAM/BAM file declares less than one reference sequence!");
+    if ((int)names.size() > M) die("The SAM/BAM file declares more reference sequences (" + std::to_string(names.size()) + ") than RSEM knows (" + std::to_string(M) + ")!");
+    if ((int)names.size() < M)
+        fprintf(stderr, "Warning: The SAM/BAM file declares less reference sequences (%d) than RSEM knows (%d)! Please make sure that you aligned your reads against transcript sequences instead of genome.\n", (int)names.size(), M);
+    std::map<std::string, int> dict;
+    for (int i = 1; i <= M; ++i) {
+        const std::string& tid = ti_type == 2 ? tr[i].seqname : tr[i].transcript_id;
+        if (!dict.emplace(tid, i).second) die("RSEM's indices might be corrupted, " + tid + " appears more than once!");
+    }
+    std::vector<int> e2i(names.size(), 0);
+    for (size_t i = 0; i < names.size(); ++i) {
+        auto it = dict.find(names[i]);
+        if (it == dict.end()) die("RSEM can not recognize reference sequence name " + names[i] + "!");
+        if (it->second < 0) die("Reference sequence name " + names[i] + " appears more than once in the SAM/BAM file!");
+        e2i[i] = it->second;
+        it->second = -1;
+    }
+    return e2i;
 }
 
 void load_groups(const std::string& path, std::vector<int>& starts) {

@@ -48,11 +48,17 @@ void load_refs(const std::string& path, bool with_seqs, RefData& out);  // Refs:
 struct TranscriptInfo {
     std::string transcript_id, transcript_name, gene_id, gene_name, seqname;
     int length = 0;
+    char strand = '+';
+    std::vector<std::pair<int, int>> exons;   // (start, end), 1-based inclusive, as the file lists them
+    int exon_length = 0;                      // sum of the exon lengths
 };
 // index 1..M; *type = 0 from a genome, 1 stand-alone transcriptome, 2 allele-specific (Transcripts.h:75)
 void load_transcripts(const std::string& path, std::vector<TranscriptInfo>& out, int* type = nullptr);
 void load_groups(const std::string& path, std::vector<int>& starts);               // GroupInfo.h:34-53
 bool load_allele_groups(const std::string& ref_name, std::vector<int>& gt, std::vector<int>& ta);  // WriteResults.h:106-123
+// Transcripts::buildMappings (Transcripts.h:105-143): BAM reference index -> transcript id 1..M (by transcript_id, by
+// seqname for an allele-specific reference), with the reference's errors and warning
+std::vector<int> map_bam_targets(const std::vector<std::string>& names, const std::vector<TranscriptInfo>& tr, int ti_type);
 
 // ---- reads (SingleRead(Q).h, PairedEndRead(Q).h, ReadReader.h) ------------------------------------
 struct ReadStore {
@@ -207,6 +213,11 @@ struct BamRecord {
     bool aux_int(const char tag[2], long long& value) const;  // bam_aux_get + bam_aux2i (0 for non-integer types)
     void set_alignment_weight(double prb);  // MAPQ + ZW:f (BamWriter.h:39-48)
 };
+uint8_t prb_to_mapq(double prb);            // bam_prb_to_mapq (sam_utils.h:72-76)
+// t[m] = the smallest float p >= 0 with prb_to_mapq(p) >= m, m = 1..100 (t[0] = 0): MAPQ(p) = #{m >= 1 : p >= t[m]}
+// for every float p >= 0, because prb_to_mapq does not decrease with p (checked for every float in [0, 2] by
+// rsem-b200-host-selftest mapq-table; from 1 on it is 100)
+std::vector<float> mapq_thresholds();
 
 class AlnReader {
 public:
@@ -236,7 +247,12 @@ private:
     bool conv_next(BamRecord& rec);
 };
 
-std::string rsem_bam_header_text(const std::string& in_text);  // SamHeader(text) + insertPG("RSEM")
+// SamHeader(text) (SamHeader.cpp:48-114) + insertPG(pg_id, pg_cl) (SamHeader.hpp:39-46), with the @SQ block replaced by
+// *sq when given (replaceSQ).  reference_pg_ids: take @PG IDs the way SamHeader::parse_line does, where a field followed
+// by others reads as ID:<value>\t<the first characters after it> (substr with an end index used as a count), and refuse
+// a @PG line without ID; otherwise the ID is the field's own value (what rsem-run-em -b has always written).
+std::string rsem_bam_header_text(const std::string& in_text, const std::string& pg_id = "RSEM", const std::string& pg_cl = "",
+                                 const std::string* sq = nullptr, bool reference_pg_ids = false);
 
 class BamWriter {
 public:
@@ -245,6 +261,7 @@ public:
     BamWriter(const BamWriter&) = delete;
     BamWriter& operator=(const BamWriter&) = delete;
     void write(const BamRecord& rec);
+    void write_encoded(const uint8_t* p, size_t n);   // records already framed as block_size + bytes
     void close();
 
 private:

@@ -43,7 +43,6 @@ struct Args {
 // reads) takes the next hit's posterior, in .dat order; all lines are written back, mates with read 1 first.
 void write_posterior_bam(const Args& a, const std::vector<TranscriptInfo>& tr, int ti_type, const HitStore& hits,
                          std::vector<double>& post, const std::vector<double>& post0, int threads) {
-    const int M = (int)tr.size() - 1;
     if (a.bamSampling) {  // one alignment (or the noise entry) per read, drawn from its posterior (EM.cpp:507-531)
         Mt engine(a.hasSeed ? a.seed : (uint32_t)time(NULL));
         if (g_verbose) printf("Begin to sample reads from their posteriors.\n");
@@ -71,25 +70,7 @@ void write_posterior_bam(const Args& a, const std::vector<TranscriptInfo>& tr, i
         if (g_verbose) printf("Sampling is finished.\n");
     }
     AlnReader in(a.inpSamF);
-    // external reference index -> internal transcript id (Transcripts::buildMappings, Transcripts.h:105-143)
-    const std::vector<std::string>& names = in.ref_names();
-    if (names.empty()) die("The SAM/BAM file declares less than one reference sequence!");
-    if ((int)names.size() > M) die("The SAM/BAM file declares more reference sequences (" + std::to_string(names.size()) + ") than RSEM knows (" + std::to_string(M) + ")!");
-    if ((int)names.size() < M)
-        fprintf(stderr, "Warning: The SAM/BAM file declares less reference sequences (%d) than RSEM knows (%d)! Please make sure that you aligned your reads against transcript sequences instead of genome.\n", (int)names.size(), M);
-    std::map<std::string, int> dict;
-    for (int i = 1; i <= M; ++i) {
-        const std::string& tid = ti_type == 2 ? tr[i].seqname : tr[i].transcript_id;
-        if (!dict.emplace(tid, i).second) die("RSEM's indices might be corrupted, " + tid + " appears more than once!");
-    }
-    std::vector<int> e2i(names.size(), 0);
-    for (size_t i = 0; i < names.size(); ++i) {
-        auto it = dict.find(names[i]);
-        if (it == dict.end()) die("RSEM can not recognize reference sequence name " + names[i] + "!");
-        if (it->second < 0) die("Reference sequence name " + names[i] + " appears more than once in the SAM/BAM file!");
-        e2i[i] = it->second;
-        it->second = -1;
-    }
+    const std::vector<int> e2i = map_bam_targets(in.ref_names(), tr, ti_type);
     BamWriter out(a.outName + ".transcript.bam", rsem_bam_header_text(in.header_text()), threads);
     const bool paired = a.read_type >= 2;
     uint64_t next_hit = 0, cnt = 0;

@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "host.hpp"
@@ -86,7 +87,52 @@ static int sidecar_dump(int argc, char** argv) {
     return 0;
 }
 
+// rsem-b200-host-selftest --mapq-table: the MAPQ threshold table rsem-tbam2gbam hands to the device against
+// prb_to_mapq for every float in [0, 2]; prints the number of floats checked and of mismatches
+static int mapq_table() {
+    const std::vector<float> t = mapq_thresholds();
+    const uint32_t hi = 0x40000000u;   // 2.0f
+    const int T = std::max(1u, std::thread::hardware_concurrency());
+    std::vector<uint64_t> bad(T, 0);
+    std::vector<std::thread> pool;
+    for (int k = 0; k < T; ++k)
+        pool.emplace_back([&, k]() {
+            for (uint64_t bits = k; bits <= hi; bits += T) {
+                float p;
+                const uint32_t b32 = (uint32_t)bits;
+                memcpy(&p, &b32, 4);
+                int m = 0;
+                for (int j = 1; j <= 100; ++j) m += p >= t[j];
+                if (m != prb_to_mapq(p)) ++bad[k];
+            }
+        });
+    for (auto& th : pool) th.join();
+    uint64_t nbad = 0;
+    for (uint64_t b : bad) nbad += b;
+    printf("%llu floats, %llu mismatches\n", (unsigned long long)hi + 1, (unsigned long long)nbad);
+    return nbad ? 1 : 0;
+}
+
+// rsem-b200-host-selftest --ti ref.ti: load_transcripts' fields, one transcript per line, tab-separated:
+// id, name, gene id, gene name, seqname, strand, length, exon length sum, then start-end of every exon
+static int ti_dump(const char* path) {
+    std::vector<TranscriptInfo> tr;
+    int type = -1;
+    load_transcripts(path, tr, &type);
+    printf("%d %d\n", (int)tr.size() - 1, type);
+    for (size_t i = 1; i < tr.size(); ++i) {
+        const TranscriptInfo& t = tr[i];
+        printf("%s\t%s\t%s\t%s\t%s\t%c\t%d\t%d", t.transcript_id.c_str(), t.transcript_name.c_str(), t.gene_id.c_str(),
+               t.gene_name.c_str(), t.seqname.c_str(), t.strand, t.length, t.exon_length);
+        for (auto& e : t.exons) printf("\t%d-%d", e.first, e.second);
+        printf("\n");
+    }
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    if (argc >= 2 && std::string(argv[1]) == "--mapq-table") return mapq_table();
+    if (argc >= 3 && std::string(argv[1]) == "--ti") return ti_dump(argv[2]);
     if (argc >= 2 && std::string(argv[1]) == "--bam-copy") return bam_copy(argc, argv);
     if (argc >= 2 && std::string(argv[1]) == "--sidecar") return sidecar_dump(argc, argv);
     if (argc != 6) {

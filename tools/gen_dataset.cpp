@@ -72,6 +72,8 @@ struct Cfg {
     double nfrac = 0.002;     // probability of an 'N' base call
     int sam = 0;              // also write <out>/aln.sam: the same reads and alignments as a SAM file the unmodified
                               // rsem-parse-alignments accepts (SamParser.h:122-265), for runs through rsem-calculate-expression
+    int genome = 0;           // place every family on a chromosome as a gene locus: r.ti of type 0 with exon structures,
+                              // and r.chrlist (rsem-tbam2gbam input).  Drawn from its own generator: the rest is unchanged
 };
 
 const char BASES[5] = {'A', 'C', 'G', 'T', 'N'};
@@ -153,6 +155,7 @@ int main(int argc, char** argv) {
         else if (k == "--omit") c.omit = atoi(v);
         else if (k == "--nfrac") c.nfrac = atof(v);
         else if (k == "--sam") c.sam = atoi(v);
+        else if (k == "--genome") c.genome = atoi(v);
         else { fprintf(stderr, "gen_dataset: unknown option %s\n", k.c_str()); return 2; }
     }
     const bool paired = c.read_type >= 2, hasQ = (c.read_type & 1);
@@ -216,9 +219,75 @@ int main(int argc, char** argv) {
         }
         fclose(f);
         f = xopen(c.out + "/ref/r.ti");
-        fprintf(f, "%d 1\n", c.M);
-        for (int t = 1; t <= c.M; ++t)
-            fprintf(f, "T%d\nG%d\nT%d\n+ %d\n1 1 %d\n\n", t, fam_of[t] + 1, t, (int)tseq[t].size(), (int)tseq[t].size());
+        if (!c.genome) {
+            fprintf(f, "%d 1\n", c.M);
+            for (int t = 1; t <= c.M; ++t)
+                fprintf(f, "T%d\nG%d\nT%d\n+ %d\n1 1 %d\n\n", t, fam_of[t] + 1, t, (int)tseq[t].size(), (int)tseq[t].size());
+        } else {
+            // genome mode: four families per chromosome, each a locus on a random strand.  An isoform is its unique
+            // prefix as one exon plus the shared body cut into 1-4 exons, with introns between; a read from the body
+            // therefore lands on the same genomic alignment from every isoform.  On '-' the transcript's 5' end is its
+            // highest coordinate: the body exons come first in the genome, the prefixes after them.
+            Rng gg(c.seed ^ 0x67656e6f6d65ull);
+            std::vector<std::vector<std::pair<int, int>>> ex(c.M + 1);
+            std::vector<int> chr_of(c.M + 1), chr_len;
+            std::vector<char> strand(c.M + 1);
+            int cursor = 0;
+            for (int fi = 0; fi < F; ++fi) {
+                if (fi % 4 == 0) { if (fi) chr_len.push_back(cursor + 1000); cursor = 1000; }
+                const int t0 = fam_start[fi], t1 = fam_start[fi + 1];
+                const int blen = (int)body[fi].size();
+                const char sd = gg.below(2) ? '-' : '+';
+                std::vector<int> cuts;   // body part boundaries in transcript order
+                const int parts = 1 + gg.below(4);
+                for (int k = 1; k < parts; ++k) cuts.push_back(gg.range(20, blen - 20));
+                std::sort(cuts.begin(), cuts.end());
+                cuts.erase(std::unique(cuts.begin(), cuts.end()), cuts.end());
+                cuts.insert(cuts.begin(), 0);
+                cuts.push_back(blen);
+                std::vector<std::pair<int, int>> body_ex, pre_ex(c.M + 1, {0, 0});
+                auto place_body = [&]() {
+                    const int n = (int)cuts.size() - 1;
+                    std::vector<std::pair<int, int>> e(n);
+                    for (int k = 0; k < n; ++k) {   // genomic order: transcript order on '+', reversed on '-'
+                        const int part = sd == '+' ? k : n - 1 - k;
+                        const int len = cuts[part + 1] - cuts[part];
+                        e[k] = {cursor + 1, cursor + len};
+                        cursor += len + gg.range(50, 2000);
+                    }
+                    body_ex = e;
+                };
+                auto place_prefixes = [&]() {
+                    for (int t = t0; t < t1; ++t)
+                        if (prefix_len[t] > 0) {
+                            pre_ex[t] = {cursor + 1, cursor + prefix_len[t]};
+                            cursor += prefix_len[t] + gg.range(50, 2000);
+                        }
+                };
+                if (sd == '+') { place_prefixes(); place_body(); }
+                else { place_body(); place_prefixes(); }
+                for (int t = t0; t < t1; ++t) {
+                    std::vector<std::pair<int, int>> e = body_ex;
+                    if (prefix_len[t] > 0) {
+                        if (sd == '+') e.insert(e.begin(), pre_ex[t]);
+                        else e.push_back(pre_ex[t]);
+                    }
+                    ex[t] = e;
+                    chr_of[t] = (int)chr_len.size() + 1;
+                    strand[t] = sd;
+                }
+            }
+            chr_len.push_back(cursor + 1000);
+            fprintf(f, "%d 0\n", c.M);
+            for (int t = 1; t <= c.M; ++t) {
+                fprintf(f, "T%d\nG%d\nchr%d\n%c %d\n%d", t, fam_of[t] + 1, chr_of[t], strand[t], (int)tseq[t].size(), (int)ex[t].size());
+                for (auto& e : ex[t]) fprintf(f, " %d %d", e.first, e.second);
+                fprintf(f, "\n\n");
+            }
+            FILE* fc = xopen(c.out + "/ref/r.chrlist");
+            for (size_t k = 0; k < chr_len.size(); ++k) fprintf(fc, "chr%zu\t%d\n", k + 1, chr_len[k]);
+            fclose(fc);
+        }
         fclose(f);
         f = xopen(c.out + "/ref/r.grp");
         for (int s : fam_start) fprintf(f, "%d\n", s);
