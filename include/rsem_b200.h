@@ -409,6 +409,48 @@ typedef struct rsem_b200_gbam_stats {
 int rsem_b200_gbam_convert(rsem_b200_ctx* ctx, const rsem_b200_gbam_tables* tables, const rsem_b200_gbam_batch* batch,
                            uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, rsem_b200_gbam_stats* stats /* may be NULL */);
 
+/* ---- rsem-bam2wig / rsem-bam2readdepth (K11, wiggle_kernels.cu) ------------------------------------------------------
+ * Replaces the per-alignment work of build_wiggles (wiggle.cpp:16-83): for every mapped record, w (bam_aux2f of its
+ * first ZW: 'f' widened, 'd', any other type 0.0; no ZW: the record adds nothing; 1.0 with no_fractional_weight, the
+ * optional fields then not read) is added to every position of every M operation of its CIGAR; D, N, = and X advance
+ * the position, every other operation neither adds nor advances.  Each position's value is the double sum, from +0.0,
+ * of its contributions in record order (x86 SSE rules for NaN and infinities); nothing is reassociated.
+ *
+ * Batch: every mapped record as BAM stores it, preceded by its u32 block_size, at data + rec_off[r].  A run is a
+ * maximal stretch of records on one target; rec_run[r] is the record's run (non-decreasing, < n_runs) and run_len[i]
+ * the target's length.  The caller checks tid and pos >= 0 (the device does not see tid).  continues = 1: run 0 is the
+ * run the previous call left resident.  keep_last = 1: the last run stays resident for the next call, which may
+ * continue it.  A call with n_runs = 0 and keep_last = 0 returns the resident run.
+ *
+ * out: the depth arrays of the runs this call finishes, concatenated in order: the previously resident run first when
+ * this call does not continue it, then runs 0 .. n_runs - 1 - keep_last.  *out_len = doubles written (<= out_cap).
+ * On a record the reference has no defined result for (an M operation that ends past run_len, an optional field of
+ * unknown type or one cut short by the record's end before the first ZW, a CIGAR past the record's end) the call
+ * returns RSEM_B200_ERR_ARG with stats->bad_record = the first such record and stats->bad_code its kind (1 M past the
+ * end, 2 unknown optional field type, 3 truncated record); the resident run is then dropped.  On every other failure
+ * (arguments, a run the device cannot allocate, CUDA errors) stats->bad_record is -1.                                                                                            */
+typedef struct rsem_b200_wig_batch {
+    uint64_t n_records, n_bytes;
+    const uint8_t* data;        /* n_bytes */
+    const uint64_t* rec_off;    /* n_records */
+    const uint32_t* rec_run;    /* n_records */
+    const uint32_t* run_len;    /* n_runs */
+    uint32_t n_runs;
+    int32_t continues;
+    int32_t keep_last;
+    int32_t no_fractional_weight;
+} rsem_b200_wig_batch;
+typedef struct rsem_b200_wig_stats {
+    double device_ms;           /* CUDA events: copies in, parse, scans, emit, sort, accumulate, copies out */
+    uint64_t blocks;            /* M operations that add */
+    uint64_t entries;           /* (tile, block) pairs */
+    int64_t bad_record;         /* -1 unless the call failed on a record */
+    int32_t bad_code;
+    int32_t reserved;
+} rsem_b200_wig_stats;
+int rsem_b200_wig_depth(rsem_b200_ctx* ctx, const rsem_b200_wig_batch* batch, double* out, uint64_t out_cap,
+                        uint64_t* out_len, rsem_b200_wig_stats* stats /* may be NULL */);
+
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);

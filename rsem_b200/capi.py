@@ -92,6 +92,18 @@ class KmerStats(C.Structure):
                 ("insert_ms", C.c_double), ("count_ms", C.c_double)]
 
 
+class WigBatch(C.Structure):
+    _fields_ = [("n_records", C.c_uint64), ("n_bytes", C.c_uint64), ("data", C.POINTER(C.c_uint8)),
+                ("rec_off", C.POINTER(C.c_uint64)), ("rec_run", C.POINTER(C.c_uint32)), ("run_len", C.POINTER(C.c_uint32)),
+                ("n_runs", C.c_uint32), ("continues", C.c_int32), ("keep_last", C.c_int32),
+                ("no_fractional_weight", C.c_int32)]
+
+
+class WigStats(C.Structure):
+    _fields_ = [("device_ms", C.c_double), ("blocks", C.c_uint64), ("entries", C.c_uint64), ("bad_record", C.c_int64),
+                ("bad_code", C.c_int32), ("reserved", C.c_int32)]
+
+
 def _dp(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
 
@@ -118,7 +130,7 @@ SYMBOLS = [
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
     "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end", "rsem_b200_kmer_shared",
-    "rsem_b200_gbam_convert",
+    "rsem_b200_gbam_convert", "rsem_b200_wig_depth",
 ]
 
 
@@ -362,6 +374,24 @@ class Context:
         self.lib.check(self.lib.dll.rsem_b200_kmer_shared(self._h, C.byref(params), _p(counts, C.c_uint64),
                                                           C.byref(stats)))
         return counts[:n], stats
+
+    def wig_depth(self, data, rec_off, rec_run, run_len, continues: bool = False, keep_last: bool = False,
+                  no_fractional_weight: bool = False, out_len: Optional[int] = None):
+        """one call of K11 -> (the depth arrays of the runs it finished, concatenated; WigStats).  data: mapped records,
+        each after its u32 block_size, at rec_off; rec_run: each record's run; run_len: each run's target length.
+        out_len: room for the output (default: the batch's positions plus any resident run's, as the caller knows)"""
+        data = _arr(np.frombuffer(bytes(data), np.uint8) if isinstance(data, (bytes, bytearray)) else data, np.uint8)
+        rec_off, rec_run, run_len = _arr(rec_off, np.uint64), _arr(rec_run, np.uint32), _arr(run_len, np.uint32)
+        cap = int(run_len.sum()) if out_len is None else out_len
+        out = np.zeros(max(cap, 1), np.float64)
+        b = WigBatch(n_records=len(rec_off), n_bytes=len(data), data=_p(data, C.c_uint8), rec_off=_p(rec_off, C.c_uint64),
+                     rec_run=_p(rec_run, C.c_uint32), run_len=_p(run_len, C.c_uint32), n_runs=len(run_len),
+                     continues=int(continues), keep_last=int(keep_last), no_fractional_weight=int(no_fractional_weight))
+        got = C.c_uint64(0)
+        stats = WigStats()
+        self.lib.check(self.lib.dll.rsem_b200_wig_depth(self._h, C.byref(b), _dp(out), C.c_uint64(cap), C.byref(got),
+                                                        C.byref(stats)))
+        return out[: got.value], stats
 
     # ---- instrumentation
     def launch_count(self) -> int:

@@ -285,6 +285,7 @@ int rsem_b200_ctx_destroy(rsem_b200_ctx* c) {
     sim_free(c);
     ci_free(c);
     gbam_free(c);
+    wig_free(c);
     if (c->model_buf) cudaFree(c->model_buf);
     if (c->stats_buf) cudaFree(c->stats_buf);
     if (c->d_stats) cudaFree(c->d_stats);
@@ -801,6 +802,18 @@ int rsem_b200_gbam_convert(rsem_b200_ctx* c, const rsem_b200_gbam_tables* t, con
     RB_ARG(b->n_units == 0 || (b->unit_rec[0] == 0 && b->unit_rec[b->n_units] == b->n_records), "unit_rec must cover the records");
     RB_CUDA(cudaSetDevice(c->device));
     return gbam_convert(c, t, b, out, out_cap, out_bytes, stats);
+}
+
+int rsem_b200_wig_depth(rsem_b200_ctx* c, const rsem_b200_wig_batch* b, double* out, uint64_t out_cap, uint64_t* out_len,
+                        rsem_b200_wig_stats* stats) {
+    if (stats) *stats = rsem_b200_wig_stats{0.0, 0, 0, -1, 0, 0};   // bad_record -1 on every other failure
+    RB_ARG(c && b && out_len && (out || out_cap == 0), "NULL argument");
+    RB_ARG(b->n_records == 0 || (b->data && b->rec_off && b->rec_run), "NULL batch array");
+    RB_ARG(b->n_runs == 0 || b->run_len, "NULL run_len");
+    RB_ARG(b->n_records == 0 || b->n_runs > 0, "records without runs");
+    RB_ARG(b->n_records < 0xffffffffull, "batch too large");
+    RB_CUDA(cudaSetDevice(c->device));
+    return wig_depth(c, b, out, out_cap, out_len, stats);
 }
 
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {

@@ -148,9 +148,38 @@ struct ClassLayout {
     bool last_profiled = false;       // the latest class-kernel launch ran with profiling on (wait_ns is current)
 };
 
+// skip_aux of htslib 1.3 (sam.c): bytes of the optional-field value whose type byte is at s, type byte included;
+// 0 = unknown type.  A 'Z' / 'H' value without its NUL before `end` gives a length that runs past `end`.  Used by K10
+// and K11 to walk a record's optional fields.
+#ifdef __CUDACC__
+__device__ __forceinline__ int aux_len(const uint8_t* s, const uint8_t* end) {
+    const uint8_t t = *s;
+    switch (t) {
+        case 'A': case 'c': case 'C': return 2;
+        case 's': case 'S': return 3;
+        case 'i': case 'I': case 'f': return 5;
+        case 'd': return 9;
+        case 'Z': case 'H': {
+            const uint8_t* q = s + 1;
+            while (q < end && *q) ++q;
+            return (int)(q - s) + 1;
+        }
+        case 'B': {
+            const uint8_t sub = s[1];
+            const int sz = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : (sub == 'i' || sub == 'I' || sub == 'f') ? 4 : 0;
+            if (sz == 0) return 0;
+            const uint32_t n = s[2] | (s[3] << 8) | (s[4] << 16) | ((uint32_t)s[5] << 24);
+            return 6 + sz * (int)n;
+        }
+    }
+    return 0;
+}
+#endif
+
 struct SimState;  // sim_kernels.cu
 struct CiState;   // ci_kernels.cu
 struct GbamState; // gbam_kernels.cu
+struct WigState;  // wiggle_kernels.cu
 
 }  // namespace rsem_b200
 
@@ -218,6 +247,7 @@ struct rsem_b200_ctx {
     rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads between sim_begin and sim_end
     rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals between ci_begin and ci_end
     rsem_b200::GbamState* gbam = nullptr;  // rsem-tbam2gbam: transcript tables and batch scratch
+    rsem_b200::WigState* wig = nullptr;    // rsem-bam2wig / rsem-bam2readdepth: the resident run and batch scratch
 
     // multi-GPU
     void* comm = nullptr;
@@ -316,5 +346,10 @@ int kmer_shared(rsem_b200_ctx* ctx, const rsem_b200_kmer_params* p, uint64_t* co
 int gbam_convert(rsem_b200_ctx* ctx, const rsem_b200_gbam_tables* t, const rsem_b200_gbam_batch* b, uint8_t* out,
                  uint64_t out_cap, uint64_t* out_bytes, rsem_b200_gbam_stats* stats);
 void gbam_free(rsem_b200_ctx* ctx);
+
+// wiggle_kernels.cu
+int wig_depth(rsem_b200_ctx* ctx, const rsem_b200_wig_batch* b, double* out, uint64_t out_cap, uint64_t* out_len,
+              rsem_b200_wig_stats* stats);
+void wig_free(rsem_b200_ctx* ctx);
 
 }  // namespace rsem_b200

@@ -77,29 +77,6 @@ __device__ __forceinline__ void flag_bad(unsigned long long* err, uint32_t unit,
     atomicMin(err, ((unsigned long long)unit << 8) | why);
 }
 
-// skip_aux of htslib 1.3 (sam.c): bytes of the field value whose type byte is at s; 0 = unknown type
-__device__ int aux_len(const uint8_t* s, const uint8_t* end) {
-    const uint8_t t = *s;
-    switch (t) {
-        case 'A': case 'c': case 'C': return 2;
-        case 's': case 'S': return 3;
-        case 'i': case 'I': case 'f': return 5;
-        case 'd': return 9;
-        case 'Z': case 'H': {
-            const uint8_t* q = s + 1;
-            while (q < end && *q) ++q;
-            return (int)(q - s) + 1;
-        }
-        case 'B': {
-            const uint8_t sub = s[1];
-            const int sz = (sub == 'c' || sub == 'C') ? 1 : (sub == 's' || sub == 'S') ? 2 : (sub == 'i' || sub == 'I' || sub == 'f') ? 4 : 0;
-            if (sz == 0) return 0;
-            return 6 + sz * (int)rd32(s + 2);
-        }
-    }
-    return 0;
-}
-
 // tr2chr (sam_utils.h:137-208), literally: the linear walk over the exons.  cig: where the CIGAR words go (unaligned),
 // nullptr to count only.  Returns the number of CIGAR operations, or -1 when the walk runs off the exons (the
 // reference's assert(i < s)).

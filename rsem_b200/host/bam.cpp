@@ -206,12 +206,13 @@ struct AlnReader::Source {
         end += (size_t)n;
         return true;
     }
+    bool lenient = false;   // read() returns false, rather than stopping, when the file ends inside the n bytes
     bool read(void* dst, size_t n) {  // exactly n bytes, false at a clean EOF before the first byte
         uint8_t* d = static_cast<uint8_t*>(dst);
         size_t got = 0;
         while (got < n) {
             if (at == end && !fill()) {
-                if (got == 0) return false;
+                if (got == 0 || lenient) return false;
                 die("Truncated BAM file!");
             }
             const size_t k = std::min(n - got, end - at);
@@ -280,13 +281,16 @@ struct AlnReader::Conv {
     }
 };
 
-AlnReader::AlnReader(const std::string& path) : src_(new Source) {
+AlnReader::AlnReader(const std::string& path, const char* tool, bool htslib_header) : src_(new Source) {
     FILE* probe = fopen(path.c_str(), "rb");
     if (!probe) die("Cannot open " + path + "! It may not exist.");
     uint8_t magic[4] = {0, 0, 0, 0};
     const size_t got = fread(magic, 1, 4, probe);
     fclose(probe);
-    if (got >= 4 && !memcmp(magic, "CRAM", 4)) die("rsem-run-em (H100): CRAM input for -b is not supported; convert it to BAM (convert-sam-for-rsem).");
+    if (got >= 4 && !memcmp(magic, "CRAM", 4)) {
+        if (!tool) die("rsem-run-em (H100): CRAM input for -b is not supported; convert it to BAM (convert-sam-for-rsem).");
+        die(std::string(tool) + " (H100): CRAM input is not supported; convert it to BAM.");
+    }
     uint8_t head[18] = {0};
     {
         FILE* p2 = fopen(path.c_str(), "rb");
@@ -304,26 +308,34 @@ AlnReader::AlnReader(const std::string& path) : src_(new Source) {
     uint8_t m4[4];
     src_->fill();
     is_bam_ = src_->end - src_->at >= 4 && !memcmp(src_->buf.data() + src_->at, "BAM\1", 4);
+    // a BAM header cut short
+    auto truncated = [htslib_header]() {
+        if (!htslib_header) die("Truncated BAM header!");
+        fprintf(stderr, "[E::bam_hdr_read] truncated bam header\n");
+        die("Cannot load SAM header!");
+    };
     if (is_bam_) {
+        src_->lenient = htslib_header;
         src_->read(m4, 4);
         uint8_t b4[4];
-        if (!src_->read(b4, 4)) die("Truncated BAM header!");
+        if (!src_->read(b4, 4)) truncated();
         const uint32_t l_text = rd_u32(b4);
         text_.resize(l_text);
-        if (l_text && !src_->read(&text_[0], l_text)) die("Truncated BAM header!");
+        if (l_text && !src_->read(&text_[0], l_text)) truncated();
         while (!text_.empty() && text_.back() == '\0') text_.pop_back();
-        if (!src_->read(b4, 4)) die("Truncated BAM header!");
+        if (!src_->read(b4, 4)) truncated();
         const uint32_t n_ref = rd_u32(b4);
         for (uint32_t i = 0; i < n_ref; ++i) {
-            if (!src_->read(b4, 4)) die("Truncated BAM header!");
+            if (!src_->read(b4, 4)) truncated();
             const uint32_t l_name = rd_u32(b4);
             std::string name(l_name, '\0');
-            if (!src_->read(&name[0], l_name)) die("Truncated BAM header!");
+            if (!src_->read(&name[0], l_name)) truncated();
             while (!name.empty() && name.back() == '\0') name.pop_back();
-            if (!src_->read(b4, 4)) die("Truncated BAM header!");
+            if (!src_->read(b4, 4)) truncated();
             ref_names_.push_back(name);
             ref_lens_.push_back(rd_u32(b4));
         }
+        src_->lenient = false;
     } else {
         // header lines up to the first alignment line (kept as the pending line)
         std::string ln;

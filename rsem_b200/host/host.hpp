@@ -221,7 +221,10 @@ std::vector<float> mapq_thresholds();
 
 class AlnReader {
 public:
-    explicit AlnReader(const std::string& path);
+    // tool: the executable named in the refusal of CRAM input (nullptr: rsem-run-em's message for -b).  htslib_header:
+    // a BAM header cut short is reported as htslib 1.3's bam_hdr_read and the reference's build_wiggles report it
+    // ("Cannot load SAM header!", wiggle.cpp:52) instead of "Truncated BAM header!"
+    explicit AlnReader(const std::string& path, const char* tool = nullptr, bool htslib_header = false);
     ~AlnReader();
     AlnReader(const AlnReader&) = delete;
     AlnReader& operator=(const AlnReader&) = delete;
@@ -271,6 +274,21 @@ private:
     void append(const uint8_t* p, size_t n);
     void flush_pending(bool all);
 };
+
+// ---- rsem-bam2wig / rsem-bam2readdepth (wiggle.cpp; the reference's wiggle.cpp:16-130) ------------------------------
+struct WigTarget {
+    std::string name;
+    uint64_t length = 0;              // target_len
+    const double* depth = nullptr;    // length values, or nullptr for the reference's empty read_depth
+};
+// What UCSCWiggleTrackWriter::process (wig) or ReadDepthWriter::process (!wig) writes for every target, in order,
+// split into chunks of about chunk_positions positions that `threads` threads format with glibc's snprintf; the
+// chunks concatenated in order are the text, whatever chunk_positions and threads are.
+void format_wiggles(const std::vector<WigTarget>& targets, bool wig, size_t chunk_positions, int threads,
+                    std::vector<std::string>& chunks);
+// build_wiggles (wiggle.cpp:16-83) with one of the two writers, onto `out` (already holding what the tool wrote first).
+// Prints the progress lines on stdout; refusals stop the run with exit status 255.
+void run_wiggles(const char* tool, const std::string& in_path, bool wig, bool no_fractional_weight, FILE* out);
 
 // boost::random::mt19937 as the reference uses it (sampling.h:12-16): engine(seed), 32-bit draws; uniform_01 = x * 2^-32
 struct Mt {

@@ -6,6 +6,7 @@
 //
 // writes <outPrefix>.{row_ptr.u64,sid.i32,pos.i32,insertL.i32,off<m>.u64,base<m>.u8,qual<m>.u8,lowq.u8} and
 // <outPrefix>.ofg (write_ofg of a synthetic conprb) plus the arrays load_ofg reads back from it.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -46,6 +47,75 @@ static int bam_copy(int argc, char** argv) {
     }
     out.close();
     printf("records %llu mapped %llu refs %zu\n", n, mapped, in.ref_names().size());
+    return 0;
+}
+
+// rsem-b200-host-selftest --bam-sort in.(sam|bam) out.bam threads
+// a stable in-memory sort of every record by (tid, pos), records without a target last, as `samtools sort` orders a
+// BAM by coordinate; the benchmark and the tests of rsem-bam2wig / rsem-bam2readdepth sort their inputs with it
+static int bam_sort(int argc, char** argv) {
+    if (argc != 5) { fprintf(stderr, "Usage: rsem-b200-host-selftest --bam-sort in out.bam threads\n"); return -1; }
+    g_io_threads = std::max(1, atoi(argv[4]));
+    AlnReader in(argv[2]);
+    std::vector<uint8_t> data;
+    std::vector<std::pair<uint64_t, uint64_t>> keys;   // (tid, pos) key, offset of the record's block_size
+    BamRecord r;
+    while (in.next(r)) {
+        const int32_t tid = r.tid();
+        const uint64_t k = tid < 0 ? ~0ull : ((uint64_t)(uint32_t)tid << 32) | (uint32_t)(r.pos() + 1);
+        keys.emplace_back(k, data.size());
+        const uint32_t n = (uint32_t)r.data.size();
+        const uint8_t b4[4] = {(uint8_t)n, (uint8_t)(n >> 8), (uint8_t)(n >> 16), (uint8_t)(n >> 24)};
+        data.insert(data.end(), b4, b4 + 4);
+        data.insert(data.end(), r.data.begin(), r.data.end());
+    }
+    std::stable_sort(keys.begin(), keys.end(), [](const std::pair<uint64_t, uint64_t>& a, const std::pair<uint64_t, uint64_t>& b) {
+        return a.first < b.first;
+    });
+    BamWriter out(argv[3], rsem_bam_header_text(in.header_text()), g_io_threads);
+    std::vector<uint8_t> buf;
+    for (const auto& k : keys) {
+        const uint8_t* p = data.data() + k.second;
+        const size_t n = 4 + (p[0] | (p[1] << 8) | (p[2] << 16) | ((size_t)p[3] << 24));
+        buf.insert(buf.end(), p, p + n);
+        if (buf.size() >= (64u << 20)) { out.write_encoded(buf.data(), buf.size()); buf.clear(); }
+    }
+    if (!buf.empty()) out.write_encoded(buf.data(), buf.size());
+    out.close();
+    printf("records %zu\n", keys.size());
+    return 0;
+}
+
+// rsem-b200-host-selftest --wig-format wig|depth chunk_positions threads values.f64 out length...
+// format_wiggles on targets t0, t1, ... whose values are read one after another from values.f64 (native doubles); a
+// length written as eN is a target of length N with the reference's empty read_depth
+static int wig_format(int argc, char** argv) {
+    if (argc < 8) { fprintf(stderr, "Usage: rsem-b200-host-selftest --wig-format wig|depth chunk threads values.f64 out length...\n"); return -1; }
+    const bool wig = std::string(argv[2]) == "wig";
+    const std::vector<char> raw = slurp(argv[5]);
+    std::vector<double> v(raw.size() / 8);
+    if (!v.empty()) memcpy(v.data(), raw.data(), v.size() * 8);
+    std::vector<WigTarget> ts;
+    size_t at = 0;
+    for (int i = 7; i < argc; ++i) {
+        WigTarget t;
+        t.name = "t" + std::to_string(i - 7);
+        const bool empty = argv[i][0] == 'e';
+        t.length = strtoull(argv[i] + (empty ? 1 : 0), nullptr, 10);
+        if (!empty && t.length) {
+            if (at + t.length > v.size()) die("--wig-format: not enough values");
+            t.depth = v.data() + at;
+            at += t.length;
+        }
+        ts.push_back(t);
+    }
+    std::vector<std::string> chunks;
+    format_wiggles(ts, wig, strtoull(argv[3], nullptr, 10), atoi(argv[4]), chunks);
+    FILE* f = fopen(argv[6], "wb");
+    if (!f) die(std::string("cannot write ") + argv[6]);
+    for (const std::string& c : chunks) fwrite(c.data(), 1, c.size(), f);
+    fclose(f);
+    printf("chunks %zu\n", chunks.size());
     return 0;
 }
 
@@ -135,6 +205,8 @@ int main(int argc, char** argv) {
     if (argc >= 3 && std::string(argv[1]) == "--ti") return ti_dump(argv[2]);
     if (argc >= 2 && std::string(argv[1]) == "--bam-copy") return bam_copy(argc, argv);
     if (argc >= 2 && std::string(argv[1]) == "--sidecar") return sidecar_dump(argc, argv);
+    if (argc >= 2 && std::string(argv[1]) == "--bam-sort") return bam_sort(argc, argv);
+    if (argc >= 2 && std::string(argv[1]) == "--wig-format") return wig_format(argc, argv);
     if (argc != 6) {
         fprintf(stderr, "Usage: rsem-b200-host-selftest imdName read_type threads seedLen outPrefix\n");
         return -1;

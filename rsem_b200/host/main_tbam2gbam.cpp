@@ -170,7 +170,7 @@ int main(int argc, char* argv[]) {
     printf("Start converting:\n");
     if (ti_type != 0) die("Genome information is not provided! RSEM cannot convert the transcript bam file!");
 
-    AlnReader in(argv[2]);
+    AlnReader in(argv[2], "rsem-tbam2gbam");
     const std::vector<int> e2i = map_bam_targets(in.ref_names(), tr, ti_type);
     std::map<std::string, int> refmap;
     const std::string sq = chrlist_sq(ref_name + ".chrlist", refmap);
