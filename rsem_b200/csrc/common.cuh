@@ -111,6 +111,7 @@ struct DevGibbs {
     int32_t* comp_tids = nullptr;  // sorted transcript ids of every component
     int32_t n_segs = 0;
     uint32_t max_len = 0;
+    bool empty_row = false;        // some read has no entry: gibbs_run refuses the matrix before any launch
 };
 
 // count reduction over NVLink peer memory (p2p.cu)

@@ -1149,10 +1149,7 @@ static int gibbs_run_serial(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, r
     RB_CUDA(cudaMemcpyAsync(h_rp.data(), g.row_ptr, (g.N1 + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
     uint64_t max_len = 1;
-    for (uint64_t i = 0; i < g.N1; ++i) {
-        max_len = std::max(max_len, h_rp[i + 1] - h_rp[i]);
-        if (h_rp[i + 1] == h_rp[i]) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
-    }
+    for (uint64_t i = 0; i < g.N1; ++i) max_len = std::max(max_len, h_rp[i + 1] - h_rp[i]);
 
     GibbsArgs a{};
     a.N1 = g.N1;
@@ -1258,6 +1255,7 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
     for (uint64_t i = 0; i < N1; ++i) {
         int32_t first = 0;
         max_len = std::max(max_len, row_ptr[i + 1] - row_ptr[i]);
+        if (row_ptr[i + 1] == row_ptr[i]) g.empty_row = true;
         for (uint64_t j = row_ptr[i]; j < row_ptr[i + 1]; ++j) {
             const int32_t t = sid[j];
             if (t < 0 || t > M) { set_error("gibbs: transcript id out of range in the .ofg matrix"); return RSEM_B200_ERR_ARG; }
@@ -1492,6 +1490,8 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
 }
 
 int gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out) {
+    // a row without entries has nothing to draw from (both kernels would fall off its empty cumulative array)
+    if (c->gibbs.empty_row) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
     const char* mode = getenv("RSEM_B200_GIBBS");   // "serial" = the one-warp-per-chain kernel (cross-check / debugging)
     if (mode && !strcmp(mode, "serial")) return gibbs_run_serial(c, p, out);
     // tiny inputs: a 624-word regeneration would span more than two sweeps (the generator runs only one sweep ahead)
