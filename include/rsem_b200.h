@@ -477,9 +477,13 @@ int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 9 */);
  * (BASELINE configs[4]).  *n = CTAs written (<= cap); 0 when the layout has no main tiles.                         */
 int rsem_b200_estep_cta_times(rsem_b200_ctx* ctx, uint64_t* out_ns, int32_t cap, int32_t* n);
 /* Where the class-layout E-step's time went in its latest main launch with profiling on (rsem_b200_set_profiling):
- * out_ns[3 i .. 3 i + 2] = { ns the consumer warps of CTA i spent blocked on staged data (summed over the warps),
+ * out_ns[8 i .. 8 i + 7] = { ns the consumer warps of CTA i spent blocked on staged data (summed over the warps),
  * ns a separate copy-issuing warp spent blocked on a free stage (0 when the consumer warps issue their own copies),
- * consumer warps of CTA i }.  *n = CTAs written (<= cap); 0 when the latest launch ran without profiling.          */
+ * consumer warps of CTA i, then in SM cycles, summed over the consumer warps: front (a batch's descriptor, ids and
+ * theta gather until theta is usable), rows (the row walk),
+ * flush (fold + reductions on the count vector), hand-over (releasing a stage -> the next stage's data seen), and
+ * last the SM cycles CTA i was busy }.  out_ns holds 8 cap entries.  *n = CTAs written (<= cap); 0 when the latest
+ * launch ran without profiling.                                                                                    */
 int rsem_b200_estep_wait_times(rsem_b200_ctx* ctx, uint64_t* out_ns, int32_t cap, int32_t* n);
 
 #ifdef __cplusplus

@@ -423,8 +423,9 @@ class Context:
 
     def estep_wait_times(self) -> np.ndarray:
         """per CTA of the latest profiled class-kernel launch: (consumer ns blocked on data summed over its warps,
-        copy-issuer ns blocked on a free stage, consumer warps); empty when that launch ran without profiling"""
-        out = np.zeros((1024, 3), np.uint64)
+        copy-issuer ns blocked on a free stage, consumer warps, SM cycles summed over the consumer warps in the phases
+        front, rows, flush and hand-over, SM cycles the CTA was busy); empty when that launch ran without profiling"""
+        out = np.zeros((1024, 8), np.uint64)
         n = C.c_int32(0)
         self.lib.check(self.lib.dll.rsem_b200_estep_wait_times(self._h, _p(out, C.c_uint64), C.c_int32(1024), C.byref(n)))
         return out[: n.value]

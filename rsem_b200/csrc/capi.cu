@@ -871,7 +871,7 @@ int rsem_b200_estep_wait_times(rsem_b200_ctx* c, uint64_t* out_ns, int32_t cap, 
     if (!L.wait_ns || !L.last_profiled || L.last_grid == 0) return 0;
     RB_CUDA(cudaSetDevice(c->device));
     const int k = std::min<int>(cap, (int)L.last_grid);
-    RB_CUDA(cudaMemcpyAsync(out_ns, L.wait_ns, (size_t)k * 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaMemcpyAsync(out_ns, L.wait_ns, (size_t)k * kWaitRecord * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
     *n = k;
     return 0;

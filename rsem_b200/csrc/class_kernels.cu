@@ -91,6 +91,33 @@ __device__ __forceinline__ void mbar_wait_timed(unsigned long long* bar, unsigne
     }
 }
 
+// %clock64 reads of the profiling build (SM cycles; one clock per SM, so the warps of a CTA share it)
+__device__ __forceinline__ long long clk() {
+    long long t;
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)::"memory");
+    return t;
+}
+// the same read behind a branch on v, so that it cannot issue before v has arrived (v is never NaN here)
+__device__ __forceinline__ long long clk_after(double v) {
+    long long t = 0;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.nan.f64 p, %1, %1;\n"
+        "@p bra RB_CLK;\n"
+        "mov.u64 %0, %%clock64;\n"
+        "RB_CLK:\n"
+        "}\n"
+        : "+l"(t)
+        : "d"(v)
+        : "memory");
+    return t;
+}
+// Phases of a consumer warp's time, in SM cycles of lane 0 (profiling build only): front = a batch's descriptor, ids
+// and theta gather until theta is usable, rows = the row walk, flush = fold + reductions on the count vector,
+// hand-over = releasing a stage -> the next stage's data seen.
+enum { kPhFront = 0, kPhRows, kPhFlush, kPhHandOver, kPhases };
+
 // ------------------------------------------------------------------------------------------------------------------
 // directory construction
 // ------------------------------------------------------------------------------------------------------------------
@@ -357,8 +384,9 @@ struct ClassArgs {
     double* count;
     const int* done_flag;
     unsigned long long* cta_ns;  // per-CTA busy time of this launch (globaltimer, ns): load-balance evidence; or nullptr
-    unsigned long long* wait_ns;  // profiling only (else nullptr): per CTA {consumer ns blocked on data, producer ns
-                                  // blocked on a free stage, consumer warps}
+    unsigned long long* wait_ns;  // profiling only (else nullptr): kWaitRecord entries per CTA {consumer ns blocked on
+                                  // data, producer ns blocked on a free stage, consumer warps, SM cycles of the consumer
+                                  // warps in the phases front, rows, flush and hand-over, SM cycles the CTA was busy}
 };
 
 struct StageDesc {  // written by the producer when it issues a tile
@@ -377,6 +405,7 @@ struct ClassSmem {
     StageDesc sd[kStages];
     double red[W + 1];
     unsigned long long wait[2];
+    unsigned long long phase[4];  // profiling: cycles per phase, summed over the consumer warps
 };
 
 __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
@@ -398,9 +427,13 @@ __device__ __forceinline__ void issue_class_tile(const ClassArgs& a, const TileR
     sd.n_batches = nb;
     sd.first_batch_mod = (unsigned)(t0.batch_begin % n_consumers);
     mbar_expect_tx(bar, b_val + b_ids + b_desc);
-    if (b_val) bulk_load(st, a.vals + vb, b_val, bar);
-    if (b_ids) bulk_load(st + b_val, a.ids + ib, b_ids, bar);
-    bulk_load(st + b_val + b_ids, a.desc + t0.batch_begin, b_desc, bar);
+    // The layout is read once per launch and is far larger than L2; theta and the count vector (a few MB) are read
+    // and added to by every batch.  With the default priority the stream's lines push those out and the theta gather
+    // and the reductions queue behind HBM; evict_first keeps them resident (C3: 3.39 -> 3.20 ms per round).
+    const unsigned long long once = l2_evict_first();
+    if (b_val) bulk_load_hint(st, a.vals + vb, b_val, bar, once);
+    if (b_ids) bulk_load_hint(st + b_val, a.ids + ib, b_ids, bar, once);
+    bulk_load_hint(st + b_val + b_ids, a.desc + t0.batch_begin, b_desc, bar, once);
 }
 
 #ifdef RB_CLASS_DEBUG
@@ -492,10 +525,12 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
 // gi: ids and theta are loaded once, the rows are walked U at a time (instruction-level parallelism across the
 // load -> product -> row sum -> reciprocal chain), the normalised weights are summed per lane and leave as ONE
 // reduction per transcript and segment.  The noise column's sum stays in the thread (count[0] is flushed per CTA).
-template <int G, int S, int U, bool TAIL>
+// PROF: ph[] takes the cycles from t0 (read by the caller before it loaded the batch's descriptor) to theta usable,
+// of the row walk and of the flush.
+template <int G, int S, int U, bool TAIL, bool PROF>
 __device__ __forceinline__ double process_batch(const double* __restrict__ bv, const int* __restrict__ bi, unsigned d,
                                                 unsigned n, unsigned nsb, bool same, const double* __restrict__ theta,
-                                                double* count, unsigned lane) {
+                                                double* count, unsigned lane, long long t0, long long (&ph)[kPhases]) {
     constexpr unsigned P = 32 / G;
     const unsigned gi = lane % P, g = lane / P;
     const bool seg_ok = gi < nsb;
@@ -517,6 +552,11 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
         th[q] = col_ok[q] ? __ldg(theta + t[q]) : 0.0;
         acc[q] = 0.0;
     }
+    if (PROF) {
+        const long long t1 = clk_after(S == 4 ? (th[0] + th[1]) + (th[2] + th[3]) : (th[0] + th[1]) + th[2]);
+        ph[kPhFront] += t1 - t0;
+        t0 = t1;
+    }
     const double* con = bv + gi;  // value (r, c) of this lane's segment at con[(r w + c) nsb]
     const unsigned row_stride = w * nsb;
     double acc0 = 0.0;
@@ -527,6 +567,11 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
     if (U > 1 && r < n)
         batch_rows<G, S, U, false, TAIL>(con + (unsigned long long)r * row_stride, row_stride, n - r, th, col_ok, coff, acc, g, w,
                                          nsb, d, bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
+    if (PROF) {
+        const long long t1 = clk_after(acc[0]);
+        ph[kPhRows] += t1 - t0;
+        t0 = t1;
+    }
     if (same && P > 1) {  // every segment of the batch adds to the same transcripts: fold them first
 #pragma unroll
         for (int q = 0; q < S; ++q) {
@@ -540,6 +585,7 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
         if (t[q] == 0) acc0 += acc[q];  // noise column (or an idle slot, whose sum is 0)
         else if (acc[q] != 0.0) red_add_f64(count + t[q], acc[q]);
     }
+    if (PROF) ph[kPhFlush] += clk() - t0;
     return acc0;
 }
 
@@ -547,7 +593,7 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
 // it waits on a stage's "empty" barrier (one arrival per consumer warp) and issues the next tile's bulk copies on its
 // "full" barrier.  Consumers wait for "full", take the batches whose global index is congruent to their warp index
 // (batches of a tile have similar shape, so the static assignment is balanced and costs no atomics), arrive on "empty".
-// PROF: wait accounting into a.wait_ns (profiling on); the kernel without it has no timer reads around the waits.
+// PROF: wait and phase accounting into a.wait_ns (profiling on); the kernel without it has no timer reads.
 // TAIL: the tiles hold only configuration-kTailCfg batches (rows with more than 127 hits), else none of them.
 template <int W, int U, bool TAIL, bool PROF>
 __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const ClassArgs a) {
@@ -556,8 +602,12 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
     if (*a.done_flag) return;
     const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     unsigned long long t_start = 0;
+    long long c_start = 0;
     if (tid == 0) {
         t_start = global_ns();
+        if (PROF) c_start = clk();
+        if (PROF)
+            for (int i = 0; i < kPhases; ++i) sm.phase[i] = 0;
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&sm.full_bar[s], 1);
             mbar_init(&sm.empty_bar[s], W);
@@ -568,6 +618,7 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
     __syncthreads();
     unsigned long long waited = 0;
     unsigned long long* const wacc = PROF ? &waited : nullptr;
+    long long ph[kPhases] = {0, 0, 0, 0};
     // tiles strided by the grid: neighbouring tiles hold batches of similar shape (the stream is sorted by degree), so
     // every CTA sees the same mix
     const unsigned k_first = blockIdx.x, k_step = gridDim.x, k_end = a.n_tiles;
@@ -587,15 +638,18 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
         }
     } else {
         unsigned it = 0;
+        long long tc = PROF ? clk() : 0;
         for (unsigned long long k = k_first; k < k_end; k += k_step, ++it) {
             const int s = it % kStages;
             mbar_wait_timed(&sm.full_bar[s], (it / kStages) & 1u, wacc);
+            if (PROF) ph[kPhHandOver] += clk() - tc;
             const unsigned char* st = sm.stage[s];
             const StageDesc sd = sm.sd[s];
             const double* s_val = reinterpret_cast<const double*>(st);
             const int* s_ids = reinterpret_cast<const int*>(st + sd.o_ids);
             const BatchDesc* s_desc = reinterpret_cast<const BatchDesc*>(st + sd.o_desc);
             for (unsigned b = (warp + W - sd.first_batch_mod) % W; b < sd.n_batches; b += W) {
+                if (PROF) tc = clk();
                 const BatchDesc bd = s_desc[b];
                 const unsigned d = (unsigned)(bd.w0 >> 48), n = (unsigned)(bd.w1 >> 40) & 255u, nsb = (unsigned)(bd.w1 >> 48) & 255u;
                 const unsigned cfg = (unsigned)(bd.w1 >> 56) & 15u;
@@ -619,24 +673,25 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
                 }
 #endif
                 if constexpr (TAIL) {
-                    acc0 += process_batch<32, 4, U, true>(bv, bi, d, n, nsb, same, a.theta, a.count, lane);
+                    acc0 += process_batch<32, 4, U, true, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph);
                 } else {
                     switch (cfg) {
-                        case 0: acc0 += process_batch<1, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 1: acc0 += process_batch<1, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 2: acc0 += process_batch<2, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 3: acc0 += process_batch<2, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 4: acc0 += process_batch<4, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 5: acc0 += process_batch<4, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 6: acc0 += process_batch<8, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 7: acc0 += process_batch<8, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 8: acc0 += process_batch<16, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 9: acc0 += process_batch<16, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        case 10: acc0 += process_batch<32, 3, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
-                        default: acc0 += process_batch<32, 4, U, false>(bv, bi, d, n, nsb, same, a.theta, a.count, lane); break;
+                        case 0: acc0 += process_batch<1, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 1: acc0 += process_batch<1, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 2: acc0 += process_batch<2, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 3: acc0 += process_batch<2, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 4: acc0 += process_batch<4, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 5: acc0 += process_batch<4, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 6: acc0 += process_batch<8, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 7: acc0 += process_batch<8, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 8: acc0 += process_batch<16, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 9: acc0 += process_batch<16, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 10: acc0 += process_batch<32, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        default: acc0 += process_batch<32, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
                     }
                 }
             }
+            if (PROF) tc = clk();
             __syncwarp();  // every lane's reads of the stage are done before lane 0 releases it
             if (lane == 0) mbar_arrive(&sm.empty_bar[s]);
         }
@@ -645,7 +700,11 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
     if (lane == 0) sm.red[warp] = acc0;
-    if (wacc && lane == 0) atomicAdd(&sm.wait[warp == W ? 1 : 0], waited);
+    if (PROF && lane == 0) {
+        atomicAdd(&sm.wait[warp == W ? 1 : 0], waited);
+        if (warp < W)
+            for (int i = 0; i < kPhases; ++i) atomicAdd(&sm.phase[i], (unsigned long long)ph[i]);
+    }
     __syncthreads();
     if (warp == 0) {
         double v = 0.0;
@@ -656,9 +715,12 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
         if (lane == 0) {
             if (a.cta_ns) a.cta_ns[blockIdx.x] = global_ns() - t_start;
             if (PROF) {
-                a.wait_ns[3 * blockIdx.x] = sm.wait[0];
-                a.wait_ns[3 * blockIdx.x + 1] = sm.wait[1];
-                a.wait_ns[3 * blockIdx.x + 2] = W;
+                unsigned long long* o = a.wait_ns + (size_t)kWaitRecord * blockIdx.x;
+                o[0] = sm.wait[0];
+                o[1] = sm.wait[1];
+                o[2] = W;
+                for (int i = 0; i < kPhases; ++i) o[3 + i] = sm.phase[i];
+                o[3 + kPhases] = (unsigned long long)(clk() - c_start);
             }
         }
     }
@@ -1036,7 +1098,7 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         }
         a.cta_ns = reinterpret_cast<unsigned long long*>(L.cta_ns);
         if (ctx->profiling && !L.wait_ns) {
-            RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.wait_ns), (size_t)ctx->sm_count * 3 * sizeof(unsigned long long)));
+            RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.wait_ns), (size_t)ctx->sm_count * kWaitRecord * sizeof(unsigned long long)));
         }
         a.wait_ns = ctx->profiling ? reinterpret_cast<unsigned long long*>(L.wait_ns) : nullptr;
         L.last_profiled = ctx->profiling;
@@ -1049,7 +1111,8 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         //   C3                      3.505  3.460  3.446  3.389  3.396  3.410  3.389  3.394  3.397  3.387  3.483  3.697
         //   C2                      0.373  0.373  0.376  0.371  0.372  0.374  0.372  0.372  0.374  0.370  0.371  0.405
         //   C5                      8.167  8.292  8.589  7.952  8.044  8.294  7.813  7.977  8.187  7.818  7.895  8.302
-        // (18 x 3 and 18 x 4 spill.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
+        // (18 x 3 and 18 x 4 spill; the sweep predates the evict_first priority of the copies, which took 15 x 2 at C3
+        // from 3.39 to 3.20 ms and has not been swept.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
         // registers), in a separate process on the same card: C3 3.519, C2 0.373, C5 8.579.
         constexpr int W = 15, U = 2;
         const size_t smem = sizeof(ClassSmem<W>);

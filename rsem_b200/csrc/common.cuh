@@ -129,6 +129,7 @@ struct P2PState {
 };
 
 // equivalence-class layout of the hit matrix for the frozen-conprb rounds (class_kernels.cu)
+constexpr int kWaitRecord = 8;  // uint64 entries per CTA in ClassLayout::wait_ns
 struct ClassLayout {
     bool built = false;
     uint64_t vals_epoch = 0;        // conprb epoch the value stream was gathered at (0 = never)
@@ -144,7 +145,8 @@ struct ClassLayout {
     uint32_t* rows = nullptr;         // sorted position -> original row
     uint32_t* long_rows = nullptr;    // original rows with more than kLongDeg hits
     uint64_t* cta_ns = nullptr;       // per-CTA busy time (ns) of the latest class-kernel launch over the main tiles
-    uint64_t* wait_ns = nullptr;      // per-CTA wait accounting of the latest profiled main launch (3 entries per CTA)
+    uint64_t* wait_ns = nullptr;      // per-CTA wait and phase accounting of the latest profiled main launch
+                                      // (kWaitRecord entries per CTA, see rsem_b200_estep_wait_times)
     uint32_t last_grid = 0;
     bool last_profiled = false;       // the latest class-kernel launch ran with profiling on (wait_ns is current)
 };

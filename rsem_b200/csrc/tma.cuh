@@ -33,6 +33,22 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, unsigned b
                  "l"(src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+// L2 eviction priority for bytes that are read once (a stream much larger than L2): their lines go first, so that
+// they do not push out the few lines every CTA reads and adds to over and over
+__device__ __forceinline__ unsigned long long l2_evict_first() {
+    unsigned long long p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+// bulk_load with an L2 eviction priority for the lines it reads
+__device__ __forceinline__ void bulk_load_hint(void* dst, const void* src, unsigned bytes, unsigned long long* bar,
+                                               unsigned long long policy) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+            smem_u32(dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+        : "memory");
+}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 

@@ -2,7 +2,11 @@
 """Where the class-layout E-step (K2) spends its time: builds a bench.py workload matrix the way bench.py does, runs a
 few frozen-conprb rounds with profiling on and prints, per persistent CTA of the last launch, its busy time, the time
 its consumer warps spent blocked on staged data (mean over the warps), the rest of the busy time (compute, i.e. not
-blocked on data) and the time a separate copy-issuing warp spent blocked on a free stage.
+blocked on data) and the time a separate copy-issuing warp spent blocked on a free stage; and, over all CTAs, the
+share of the consumer warps' busy time (SM cycles) spent in each phase of a batch: front (descriptor, ids and theta
+gather until theta is usable), rows (the row walk), flush (fold +
+reductions) and hand-over (releasing a stage -> the next stage's data seen); "other" is the rest (loop control, timer
+reads, the time before the first and after the last tile).
 
   python tools/k2_anatomy.py [--workload C3] [--scale 1.0] [--per-cta]
 
@@ -73,12 +77,18 @@ def main():
     warps = w[:, 2]
     data_wait = w[:, 0] / warps / 1e3  # mean over the CTA's consumer warps
     compute = busy - data_wait
+    warp_cycles = float((warps * w[:, 7]).sum())  # busy cycles of all consumer warps
+    shares = {k: round(float(w[:, 3 + i].sum()) / warp_cycles, 4) for i, k in enumerate(("front", "rows", "flush", "hand_over"))}
+    shares["other"] = round(1.0 - sum(shares.values()), 4)
     out = {"workload": args.workload, "reads": N, "hits": H, "gpu": torch.cuda.get_device_name(0),
            "k2_ms_per_launch_with_profiling": round(k2_ms / k2_n, 4), "ctas": int(busy.size),
            "consumer_warps_per_cta": int(warps[0]), "bytes_per_round": info["bytes_per_round"],
            "busy_us": _summary(busy), "data_wait_us_per_warp": _summary(data_wait), "compute_us_per_warp": _summary(compute),
            "producer_wait_us": _summary(w[:, 1] / 1e3),
            "data_wait_share_of_busy": round(float(data_wait.sum() / busy.sum()), 4),
+           "producer_wait_share_of_busy": round(float((w[:, 1] / 1e3).sum() / busy.sum()), 4),
+           "phase_share_of_warp_cycles": shares,
+           "sm_cycles_per_ns": round(float(w[:, 7].sum() / (busy.sum() * 1e3)), 3),
            "note": "last profiled launch; data wait = time a consumer warp blocked on its staged data (mean over the CTA's "
                    "warps), compute = busy - data wait; profiling adds %globaltimer reads around every wait"}
     if args.per_cta:
