@@ -487,3 +487,219 @@ void ro_gibbs_chain(uint64_t N1, const uint64_t* row_ptr, const int32_t* sid, co
     }
     free(counts); free(z); free(theta); free(tpm); free(fpkm); free(arr);
 }
+
+/* ------------------------------------------------------------------------------------------ */
+/* Phase II of rsem-calculate-credibility-intervals (calcCI.cpp:218-385)                        */
+
+/* ascending sort of n floats: LSD radix over the order-preserving unsigned image of the bits.
+ * For the finite values without -0.0 that Phase I produces it orders exactly as operator<.     */
+static void ci_sort(float* v, uint32_t* a, uint32_t* b, int64_t n) {
+    if (n <= 32) { /* insertion sort by operator< for short rows */
+        for (int64_t i = 1; i < n; ++i) {
+            const float x = v[i];
+            int64_t j = i;
+            for (; j > 0 && x < v[j - 1]; --j) v[j] = v[j - 1];
+            v[j] = x;
+        }
+        return;
+    }
+    for (int64_t i = 0; i < n; ++i) {
+        uint32_t u;
+        memcpy(&u, &v[i], 4);
+        a[i] = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    }
+    for (int shift = 0; shift < 32; shift += 8) {
+        int64_t cnt[257] = {0};
+        for (int64_t i = 0; i < n; ++i) ++cnt[((a[i] >> shift) & 0xff) + 1];
+        for (int d = 0; d < 256; ++d) cnt[d + 1] += cnt[d];
+        for (int64_t i = 0; i < n; ++i) b[cnt[(a[i] >> shift) & 0xff]++] = a[i];
+        uint32_t* t = a; a = b; b = t;
+    }
+    for (int64_t i = 0; i < n; ++i) {
+        const uint32_t u = (a[i] & 0x80000000u) ? (a[i] & 0x7fffffffu) : ~a[i];
+        memcpy(&v[i], &u, 4);
+    }
+}
+
+/* calcCI on s, sorted in place: out = lb, ub, cqv (calcCI.cpp:218-284) */
+static void ci_calc(float* s, uint32_t* a, uint32_t* b, int n, int threshold, float* out) {
+    ci_sort(s, a, b, n);
+    int p = 0, q = n - 1, newp, newq = n - 1;
+    /* q: the first element of the run of ties at the top that still leaves at most threshold above it */
+    do {
+        q = newq;
+        while (newq > 0 && s[newq - 1] == s[newq]) newq--;
+        newq--;
+    } while (newq >= 0 && n - (newq + 1) <= threshold);
+    int outside = n - (q + 1);
+    float lb = (float)-1e30, ub = (float)1e30;
+    do {
+        const float width = s[q] - s[p], best = ub - lb;
+        if (width < best) {
+            lb = s[p];
+            ub = s[q];
+        }
+        newp = p;
+        while (newp < n - 1 && s[newp] == s[newp + 1]) newp++;
+        newp++;
+        if (newp <= threshold) {
+            outside += newp - p;
+            p = newp;
+            while (outside > threshold && q < n - 1) {
+                newq = q + 1;
+                while (newq < n - 1 && s[newq] == s[newq + 1]) newq++;
+                outside -= newq - q;
+                q = newq;
+            }
+        } else {
+            p = newp;
+        }
+    } while (p <= threshold);
+    /* Tukey's hinges: a float sum halved in double, rounded back to float */
+    const int quo = n / 4, res = n % 4;
+    float q1, q3;
+    if (res == 0) {
+        const float x = s[quo - 1] + s[quo], y = s[3 * quo - 1] + s[3 * quo];
+        q1 = (float)((double)x / 2.0);
+        q3 = (float)((double)y / 2.0);
+    } else if (res == 3) {
+        const float x = s[quo] + s[quo + 1], y = s[3 * quo + 1] + s[3 * quo + 2];
+        q1 = (float)((double)x / 2.0);
+        q3 = (float)((double)y / 2.0);
+    } else {
+        q1 = s[quo];
+        q3 = s[3 * quo];
+    }
+    const float d = q3 - q1, sum = q3 + q1;
+    out[0] = lb;
+    out[1] = ub;
+    out[2] = d > 0.0f ? d / sum : 0.0f;
+}
+
+typedef struct ci_bufs {
+    float *t, *f, *gt, *gf, *it, *itf;
+    uint32_t *a, *b;
+} ci_bufs;
+
+static void ci_bufs_alloc(ci_bufs* w, int64_t n) {
+    float** fs[6] = {&w->t, &w->f, &w->gt, &w->gf, &w->it, &w->itf};
+    for (int i = 0; i < 6; ++i) *fs[i] = (float*)calloc((size_t)n, sizeof(float));
+    w->a = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)n);
+    w->b = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)n);
+}
+
+static void ci_bufs_free(ci_bufs* w) {
+    free(w->t); free(w->f); free(w->gt); free(w->gf); free(w->it); free(w->itf); free(w->a); free(w->b);
+}
+
+/* an isoform ends before allele end_j (calcCI.cpp:321-330, 364-373): the running sums, sorted in place, when it has
+ * several alleles, else the intervals of its one allele.  The sort happens even when the result is not kept (keep = 0):
+ * the later isoforms of the range add onto the sorted sums. */
+static void ci_finish_isoform(ci_bufs* w, int64_t n, int threshold, int tid, int curaid, int end_j, int keep,
+                              const float* tr_out, float* iso_out) {
+    float dropped[6];
+    float* o = keep ? iso_out + (size_t)tid * 6 : dropped;
+    if (end_j - curaid > 1) {
+        ci_calc(w->it, w->a, w->b, (int)n, threshold, o);
+        ci_calc(w->itf, w->a, w->b, (int)n, threshold, o + 3);
+    } else {
+        memcpy(o, tr_out + (size_t)(curaid - 1) * 6, 6 * sizeof(float));
+    }
+}
+
+/* genes [g0, g1) with their transcripts; with isoforms, the running isoform sums of one Phase II range.  iso_last[tid]
+ * is the range whose result the isoform keeps: the one holding its last allele */
+static void ci_range(int64_t n, const float* samples, const float* l_bars, const int32_t* gene_start,
+                     const int32_t* iso_of, const int32_t* iso_last, int32_t part, int32_t g0, int32_t g1,
+                     int32_t threshold, float* tr_out, float* gene_out, float* iso_out, ci_bufs* w) {
+    int curtid = -1, curaid = -1;
+    if (iso_of) {
+        memset(w->it, 0, sizeof(float) * (size_t)n);
+        memset(w->itf, 0, sizeof(float) * (size_t)n);
+    }
+    for (int32_t g = g0; g < g1; ++g) {
+        const int b = gene_start[g], e = gene_start[g + 1];
+        memset(w->gt, 0, sizeof(float) * (size_t)n);
+        memset(w->gf, 0, sizeof(float) * (size_t)n);
+        for (int j = b; j < e; ++j) {
+            if (iso_of && curtid != iso_of[j]) {
+                if (curtid >= 0)
+                    ci_finish_isoform(w, n, threshold, curtid, curaid, j, iso_last[curtid] == part, tr_out, iso_out);
+                curtid = iso_of[j];
+                curaid = j;
+            }
+            const float* row = samples + (size_t)(j - 1) * (size_t)n;
+            for (int64_t k = 0; k < n; ++k) {
+                w->t[k] = row[k];
+                w->f[k] = (float)(1e3 / (double)l_bars[k] * (double)row[k]);
+                if (iso_of) {
+                    w->it[k] += w->t[k];
+                    w->itf[k] += w->f[k];
+                }
+                w->gt[k] += w->t[k];
+                w->gf[k] += w->f[k];
+            }
+            ci_calc(w->t, w->a, w->b, (int)n, threshold, tr_out + (size_t)(j - 1) * 6);
+            ci_calc(w->f, w->a, w->b, (int)n, threshold, tr_out + (size_t)(j - 1) * 6 + 3);
+        }
+        if (e - b > 1) {
+            ci_calc(w->gt, w->a, w->b, (int)n, threshold, gene_out + (size_t)g * 6);
+            ci_calc(w->gf, w->a, w->b, (int)n, threshold, gene_out + (size_t)g * 6 + 3);
+        } else {
+            memcpy(gene_out + (size_t)g * 6, tr_out + (size_t)(b - 1) * 6, 6 * sizeof(float));
+        }
+    }
+    if (iso_of && curtid >= 0)
+        ci_finish_isoform(w, n, threshold, curtid, curaid, gene_start[g1], iso_last[curtid] == part, tr_out, iso_out);
+}
+
+void ro_ci_phase2(int32_t M, int64_t n, const float* samples, const float* l_bars, int32_t n_genes,
+                  const int32_t* gene_start, int32_t n_isoforms, const int32_t* isoform_start, int32_t n_parts,
+                  const int32_t* part_gene_start, int32_t threshold, float* tr_out, float* gene_out, float* iso_out,
+                  int32_t n_threads) {
+#ifdef _OPENMP
+    if (n_threads < 1) n_threads = omp_get_max_threads();
+#else
+    n_threads = 1;
+#endif
+    if (n_isoforms <= 0 || !isoform_start) { /* every gene stands alone */
+#ifdef _OPENMP
+#pragma omp parallel num_threads(n_threads)
+#endif
+        {
+            ci_bufs w;
+            ci_bufs_alloc(&w, n);
+#ifdef _OPENMP
+#pragma omp for schedule(dynamic, 16)
+#endif
+            for (int32_t g = 0; g < n_genes; ++g)
+                ci_range(n, samples, l_bars, gene_start, NULL, NULL, 0, g, g + 1, threshold, tr_out, gene_out, NULL, &w);
+            ci_bufs_free(&w);
+        }
+        return;
+    }
+    int32_t* iso_of = (int32_t*)malloc(sizeof(int32_t) * ((size_t)M + 1));
+    int32_t* iso_last = (int32_t*)malloc(sizeof(int32_t) * (size_t)n_isoforms);
+    int32_t* part_of = (int32_t*)malloc(sizeof(int32_t) * ((size_t)M + 1));
+    for (int32_t i = 0; i < n_isoforms; ++i)
+        for (int32_t j = isoform_start[i]; j < isoform_start[i + 1]; ++j) iso_of[j] = i;
+    for (int32_t p = 0; p < n_parts; ++p)
+        for (int32_t g = part_gene_start[p]; g < part_gene_start[p + 1]; ++g)
+            for (int32_t j = gene_start[g]; j < gene_start[g + 1]; ++j) part_of[j] = p;
+    for (int32_t i = 0; i < n_isoforms; ++i) iso_last[i] = part_of[isoform_start[i + 1] - 1];
+#ifdef _OPENMP
+#pragma omp parallel num_threads(n_threads)
+#endif
+    {
+        ci_bufs w;
+        ci_bufs_alloc(&w, n);
+#ifdef _OPENMP
+#pragma omp for schedule(dynamic, 1)
+#endif
+        for (int32_t p = 0; p < n_parts; ++p)
+            ci_range(n, samples, l_bars, gene_start, iso_of, iso_last, p, part_gene_start[p], part_gene_start[p + 1],
+                     threshold, tr_out, gene_out, iso_out, &w);
+        ci_bufs_free(&w);
+    }
+    free(iso_of); free(iso_last); free(part_of);
+}

@@ -120,3 +120,22 @@ class Oracle:
         theta = c64(theta).copy()
         self.dll.ro_polish_theta(C.c_int32(len(theta) - 1), _p(theta, C.c_double), _p(c64(eel), C.c_double), _p(c64(mw), C.c_double))
         return theta
+
+    def ci_phase2(self, samples, l_bars, gene_start, threshold, isoform_start=None, part_gene_start=None, n_threads=0):
+        """Phase II of rsem-calculate-credibility-intervals on samples, M x n float32 TPMs (transcript-major).
+        -> (transcripts M x 6, genes x 6, isoforms x 6) float32: TPM lb ub cqv, FPKM lb ub cqv"""
+        samples = np.ascontiguousarray(samples, np.float32)
+        l_bars = np.ascontiguousarray(l_bars, np.float32)
+        gene_start = np.ascontiguousarray(gene_start, np.int32)
+        M, n = samples.shape
+        m = len(gene_start) - 1
+        assert len(l_bars) == n and gene_start[-1] == M + 1
+        iso = None if isoform_start is None else np.ascontiguousarray(isoform_start, np.int32)
+        parts = np.ascontiguousarray([0, m] if part_gene_start is None else part_gene_start, np.int32)
+        n_iso = 0 if iso is None else len(iso) - 1
+        tr, ge, io = np.zeros((M, 6), np.float32), np.zeros((m, 6), np.float32), np.zeros((n_iso, 6), np.float32)
+        self.dll.ro_ci_phase2(C.c_int32(M), C.c_int64(n), _p(samples, C.c_float), _p(l_bars, C.c_float), C.c_int32(m),
+                              _p(gene_start, C.c_int32), C.c_int32(n_iso), _p(iso, C.c_int32), C.c_int32(len(parts) - 1),
+                              _p(parts, C.c_int32), C.c_int32(threshold), _p(tr, C.c_float), _p(ge, C.c_float),
+                              _p(io, C.c_float) if n_iso else None, C.c_int32(n_threads))
+        return tr, ge, io

@@ -15,6 +15,7 @@ import tarfile
 
 import pytest
 
+import ci_phase2
 import rsem_files as rf
 
 pytestmark = pytest.mark.gpu
@@ -39,14 +40,7 @@ def _dataset(tmp_path, key, name, nsamples, threads, seed=7, gibbs_extra=(), all
     shutil.rmtree(tmp_path / "x")
     M = int(open(d / "ref" / "r.ti").readline().split()[0])
     if alleles:  # alleles 2k - 1 and 2k form isoform k where both lie in one gene; otherwise an allele is its own isoform
-        grp = [int(x) for x in open(d / "ref" / "r.grp").read().split()]
-        ta = [1]
-        while ta[-1] <= M:
-            a = ta[-1]
-            ta.append(a + 2 if a + 1 <= M and not any(a < g <= a + 1 for g in grp) else a + 1)
-        gt = [ta.index(g) for g in grp]
-        open(d / "ref" / "r.ta", "w").write("\n".join(map(str, ta)) + "\n")
-        open(d / "ref" / "r.gt", "w").write("\n".join(map(str, gt)) + "\n")
+        ci_phase2.write_allele_tables(d / "ref", M)
     extra = list(gibbs_extra)
     if "--prior" in extra:
         open(d / "prior.txt", "w").write("".join(f"{0.1 + (i % 7) * 0.4:.2f}\n" for i in range(M)))
