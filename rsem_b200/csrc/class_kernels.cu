@@ -16,7 +16,7 @@
 //   * ids are stored once per segment (4 B per hit / rows per segment) and row pointers disappear (a batch
 //     descriptor of 16 B replaces them): ~9.2 B per hit at C3 instead of 12.8;
 //   * batches are staged by 1-D bulk-async copies (TMA) into a 3-stage shared-memory ring per persistent CTA, as in the
-//     row kernel; warps claim batches from a shared-memory counter, no CTA-wide barrier per tile;
+//     row kernel; each CTA claims tiles from a counter in global memory, no CTA-wide barrier per tile;
 //   * rows longer than kLongDeg hits (never produced behind RSEM's aligner caps of 200) are left out of the
 //     layout and handled by their own launch on the CSR stream - they no longer demote the whole matrix.
 //
@@ -383,6 +383,7 @@ struct ClassArgs {
     const double* theta;
     double* count;
     const int* done_flag;
+    unsigned* claim;             // {next tile to claim, CTAs done}: 0 between launches (the last CTA to finish resets it)
     unsigned long long* cta_ns;  // per-CTA busy time of this launch (globaltimer, ns): load-balance evidence; or nullptr
     unsigned long long* wait_ns;  // profiling only (else nullptr): kWaitRecord entries per CTA {consumer ns blocked on
                                   // data, producer ns blocked on a free stage, consumer warps, SM cycles of the consumer
@@ -393,9 +394,10 @@ struct StageDesc {  // written by the producer when it issues a tile
     unsigned long long val_base;  // index of the first staged value (val_begin rounded down to 16 B)
     unsigned long long id_base;
     unsigned o_ids, o_desc;       // byte offsets of the id and descriptor slices inside the stage
-    unsigned n_batches;
+    unsigned n_batches;           // kNoTile: no tile left, the consumers leave
     unsigned first_batch_mod;     // (global index of the tile's first batch) % consumer warps
 };
+constexpr unsigned kNoTile = 0xffffffffu;
 
 template <int W>
 struct ClassSmem {
@@ -590,9 +592,11 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
 }
 
 // W consumer warps + 1 producer warp per CTA (one CTA per SM).  The producer's lane 0 keeps the 3-stage ring full:
-// it waits on a stage's "empty" barrier (one arrival per consumer warp) and issues the next tile's bulk copies on its
-// "full" barrier.  Consumers wait for "full", take the batches whose global index is congruent to their warp index
-// (batches of a tile have similar shape, so the static assignment is balanced and costs no atomics), arrive on "empty".
+// it claims the next tile from a counter in global memory, waits on a stage's "empty" barrier (one arrival per
+// consumer warp) and issues the tile's bulk copies on its "full" barrier; when no tile is left it hands the consumers
+// a stage without tile instead.  Consumers wait for "full", take the batches whose global index is congruent to their
+// warp index (batches of a tile have similar shape, so the static assignment is balanced and costs no atomics), arrive
+// on "empty".
 // PROF: wait and phase accounting into a.wait_ns (profiling on); the kernel without it has no timer reads.
 // TAIL: the tiles hold only configuration-kTailCfg batches (rows with more than 127 hits), else none of them.
 template <int W, int U, bool TAIL, bool PROF>
@@ -619,32 +623,45 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
     unsigned long long waited = 0;
     unsigned long long* const wacc = PROF ? &waited : nullptr;
     long long ph[kPhases] = {0, 0, 0, 0};
-    // tiles strided by the grid: neighbouring tiles hold batches of similar shape (the stream is sorted by degree), so
-    // every CTA sees the same mix
-    const unsigned k_first = blockIdx.x, k_step = gridDim.x, k_end = a.n_tiles;
+    // Tiles are claimed in stream order by whichever CTA has a stage to fill next.  Neighbouring tiles hold batches of
+    // similar shape (the stream is sorted by degree), so every CTA sees the same mix, and a CTA whose tiles go slower
+    // (SMs do not all see the same memory latency) takes fewer of them: the CTAs finish within about a tile of each
+    // other, where a fixed stride over the grid left the launch waiting on the slowest CTA.
     double acc0 = 0.0;
     if (warp == W) {
         if (lane == 0) {
-            unsigned it = 0;
-            for (unsigned long long k = k_first; k < k_end; k += k_step, ++it) {
+            unsigned k = atomicAdd(&a.claim[0], 1u);
+            for (unsigned it = 0;; ++it) {
                 const int s = it % kStages;
-                const TileRec t0 = a.tile[k], t1 = a.tile[k + 1];  // in flight while the stage is still in use
+                const bool last = k >= a.n_tiles;
+                TileRec t0{}, t1{};
+                if (!last) {
+                    t0 = a.tile[k];  // in flight while the stage is still in use
+                    t1 = a.tile[k + 1];
+                }
+                const unsigned k_next = last ? k : atomicAdd(&a.claim[0], 1u);  // likewise
                 if (it >= (unsigned)kStages) {
                     mbar_wait_timed(&sm.empty_bar[s], ((it / kStages) - 1u) & 1u, wacc);
                     fence_proxy_async();  // the consumers' generic-proxy reads precede the async-proxy refill
                 }
+                if (last) {
+                    sm.sd[s].n_batches = kNoTile;
+                    mbar_arrive(&sm.full_bar[s]);
+                    break;
+                }
                 issue_class_tile(a, t0, t1, sm.stage[s], &sm.full_bar[s], sm.sd[s], W);
+                k = k_next;
             }
         }
     } else {
-        unsigned it = 0;
         long long tc = PROF ? clk() : 0;
-        for (unsigned long long k = k_first; k < k_end; k += k_step, ++it) {
+        for (unsigned it = 0;; ++it) {
             const int s = it % kStages;
             mbar_wait_timed(&sm.full_bar[s], (it / kStages) & 1u, wacc);
             if (PROF) ph[kPhHandOver] += clk() - tc;
             const unsigned char* st = sm.stage[s];
             const StageDesc sd = sm.sd[s];
+            if (sd.n_batches == kNoTile) break;
             const double* s_val = reinterpret_cast<const double*>(st);
             const int* s_ids = reinterpret_cast<const int*>(st + sd.o_ids);
             const BatchDesc* s_desc = reinterpret_cast<const BatchDesc*>(st + sd.o_desc);
@@ -666,9 +683,9 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
                     if (!bad)
                         for (unsigned long long i = lane; i < nv; i += 32) nan = nan || (bv[i] != bv[i]) || bv[i] < 0.0 || bv[i] > 1.0;
                     if ((bad || __any_sync(0xffffffffu, nan)) && lane == 0 && atomicCAS(&g_dbg_flag, 0, 1) == 0)
-                        printf("CLASSDBG cta %u warp %u it %u s %d k %llu b %u/%u bad %d | d %u n %u nsb %u cfg %u vo %llu nv %llu o_ids %u o_desc %u "
+                        printf("CLASSDBG cta %u warp %u it %u s %d b %u/%u bad %d | d %u n %u nsb %u cfg %u vo %llu nv %llu o_ids %u o_desc %u "
                                "val_base %llu id_base %llu fbm %u | w0 %llx w1 %llx\n",
-                               blockIdx.x, warp, it, s, k, b, sd.n_batches, (int)bad, d, n, nsb, cfg, vo, nv, sd.o_ids, sd.o_desc, sd.val_base,
+                               blockIdx.x, warp, it, s, b, sd.n_batches, (int)bad, d, n, nsb, cfg, vo, nv, sd.o_ids, sd.o_desc, sd.val_base,
                                sd.id_base, sd.first_batch_mod, bd.w0, bd.w1);
                 }
 #endif
@@ -712,6 +729,10 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
         if (lane == 0 && v != 0.0) red_add_f64(a.count, v);
+        if (lane == 0 && atomicAdd(&a.claim[1], 1u) == gridDim.x - 1u) {  // every CTA has made its last claim
+            a.claim[0] = 0;
+            a.claim[1] = 0;
+        }
         if (lane == 0) {
             if (a.cta_ns) a.cta_ns[blockIdx.x] = global_ns() - t_start;
             if (PROF) {
@@ -826,7 +847,7 @@ void class_free(rsem_b200_ctx* ctx) {
     ClassLayout& L = ctx->cls;
     block_free(ctx, L.vals); block_free(ctx, L.ids); block_free(ctx, L.desc); block_free(ctx, L.tile); block_free(ctx, L.batch_first);
     block_free(ctx, L.fseg_first); block_free(ctx, L.rows); block_free(ctx, L.long_rows); block_free(ctx, L.cta_ns);
-    block_free(ctx, L.wait_ns);
+    block_free(ctx, L.wait_ns); block_free(ctx, L.claim);
     L = ClassLayout{};
 }
 
@@ -1053,6 +1074,8 @@ int class_build(rsem_b200_ctx* ctx) {
     RB_CUDA(cudaGetLastError());
     RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.vals), ((size_t)L.n_vals + 32) * sizeof(double)));
     RB_CUDA(cudaMemsetAsync(L.vals + L.n_vals, 0, 32 * sizeof(double), st));
+    RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.claim), 2 * sizeof(unsigned)));
+    RB_CUDA(cudaMemsetAsync(L.claim, 0, 2 * sizeof(unsigned), st));
     RB_CUDA(cudaStreamSynchronize(st));
     pt.mark("tiles, descriptors, ids");
     sc.keep(rows_s);
@@ -1089,6 +1112,7 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
     a.theta = ctx->theta;
     a.count = ctx->k2_target;
     a.done_flag = ctx->done_flag;
+    a.claim = L.claim;
     L.last_grid = 0;
     if (L.n_tiles_main) {  // rows of <= 127 hits; the per-CTA busy and wait times come from this launch
         a.tile = static_cast<const TileRec*>(L.tile);
@@ -1104,7 +1128,7 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         L.last_profiled = ctx->profiling;
         const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
         L.last_grid = grid;
-        // 15 consumer warps x 2 rows in flight per lane (102 registers, no spills).  Without the tail code more warps
+        // 15 consumer warps x 2 rows in flight per lane (98 registers, no spills).  Without the tail code more warps
         // fit and hide more of a batch's latency (ids -> theta gather -> values -> row sums); 18 warps are no faster.
         // Measured on H100 80GB HBM3 at 700 W, ms per round, median of 3 alternating runs in one process:
         //   consumer warps x rows:  11x2   11x3   11x4   14x2   14x3   14x4   15x2   15x3   15x4   18x2   18x3   18x4

@@ -144,6 +144,7 @@ struct ClassLayout {
     uint32_t* fseg_first = nullptr;   // first sorted row position of every segment (final order)
     uint32_t* rows = nullptr;         // sorted position -> original row
     uint32_t* long_rows = nullptr;    // original rows with more than kLongDeg hits
+    uint32_t* claim = nullptr;        // {next tile, CTAs done} of the class-kernel launch in flight; 0 between launches
     uint64_t* cta_ns = nullptr;       // per-CTA busy time (ns) of the latest class-kernel launch over the main tiles
     uint64_t* wait_ns = nullptr;      // per-CTA wait and phase accounting of the latest profiled main launch
                                       // (kWaitRecord entries per CTA, see rsem_b200_estep_wait_times)
