@@ -219,7 +219,38 @@ typedef struct rsem_b200_gibbs_out {
 
 int rsem_b200_gibbs_upload(rsem_b200_ctx* ctx, uint64_t N1, uint64_t E, int32_t M, const uint64_t* row_ptr,
                            const int32_t* sid, const double* conprb);
+/* = rsem_b200_gibbs_run_chains followed by rsem_b200_gibbs_sum_chains */
 int rsem_b200_gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* params, rsem_b200_gibbs_out* out);
+
+/* ---- Gibbs over several GPUs: the reference's threads are independent chains (Gibbs.cpp:265-353), so a run's chains can
+ * be split into contiguous ranges, one per device, and their per-chain sums added up on the host in chain order.
+ * A chain's draws depend only on its own seed and sample count, never on the other chains of the call.               */
+/* device time and shape of one rsem_b200_gibbs_run_chains call */
+typedef struct rsem_b200_gibbs_stats {
+    double device_ms;      /* CUDA events around the sampler's launches                                         */
+    int32_t worker_ctas;   /* worker CTAs per chain of the component-parallel kernel; 0 when the serial kernel ran */
+    int32_t launches;      /* kernel launches (waves of chains)                                                 */
+} rsem_b200_gibbs_stats;
+/* Runs the chains params describes (any contiguous range of a run: the caller passes the sub-arrays of chain_samples /
+ * chain_seeds).  count_vectors: as rsem_b200_gibbs_out.count_vectors, for these chains.  chain_acc: n_chains blocks of
+ * 4 (M + 1) + n_genes doubles in chain order, each holding one chain's sum_c, sum_c2, sum_tpm, sum_fpkm (M + 1 each)
+ * and sum_gene_c2 (n_genes).  stats may be NULL.                                                                    */
+int rsem_b200_gibbs_run_chains(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* params, int32_t* count_vectors,
+                               double* chain_acc, rsem_b200_gibbs_stats* stats);
+/* out's sums (count_vectors is not touched) = the params->n_chains blocks of chain_acc added up in chain order
+ * (Gibbs.cpp:372-397).  Pure host arithmetic (no device needed).                                                    */
+int rsem_b200_gibbs_sum_chains(const rsem_b200_gibbs_params* params, const double* chain_acc, rsem_b200_gibbs_out* out);
+/* Contiguous chain ranges for n_parts devices: part i runs chains [bounds[i], bounds[i + 1]).  A chain costs
+ * burnin + 1 + (chain_samples[t] - 1) gap sweeps; bound i is the chain boundary whose prefix of sweeps is nearest to
+ * i / n_parts of the total (the lower one on a tie), every part at least one chain while chains are left.  More parts
+ * than chains: the surplus parts are empty.  Pure host arithmetic; bounds has n_parts + 1 entries.                    */
+int rsem_b200_gibbs_split_chains(int32_t n_chains, const int32_t* chain_samples, int32_t burnin, int32_t gap,
+                                 int32_t n_parts, int32_t* bounds);
+/* Gives dst (any device, another context) the matrix uploaded to src with rsem_b200_gibbs_upload, component layout
+ * included, by device-to-device copies (over NVLink where the two devices can map each other's memory): the host-side
+ * component analysis and the row permutation run once, on src.  dst's previous matrix is released.  A src without a
+ * completed upload, or src == dst, is refused with RSEM_B200_ERR_ARG.                                                */
+int rsem_b200_gibbs_upload_from(rsem_b200_ctx* dst, const rsem_b200_ctx* src);
 
 typedef struct rsem_b200_sim_stats rsem_b200_sim_stats;
 

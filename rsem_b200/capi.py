@@ -53,6 +53,10 @@ class GibbsOut(C.Structure):
                 ("sum_fpkm", C.POINTER(C.c_double)), ("sum_gene_c2", C.POINTER(C.c_double))]
 
 
+class GibbsStats(C.Structure):
+    _fields_ = [("device_ms", C.c_double), ("worker_ctas", C.c_int32), ("launches", C.c_int32)]
+
+
 class SimParams(C.Structure):
     _fields_ = [("model_type", C.c_int32), ("M", C.c_int32), ("seed", C.c_uint32), ("exact_body", C.c_int32),
                 ("N", C.c_uint64), ("window_words", C.c_uint64), ("theta_cdf", C.POINTER(C.c_double)),
@@ -130,7 +134,8 @@ SYMBOLS = [
     "rsem_b200_set_estep_variant", "rsem_b200_class_layout_info", "rsem_b200_shard_reads",
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
     "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end", "rsem_b200_kmer_shared",
-    "rsem_b200_gbam_convert", "rsem_b200_wig_depth",
+    "rsem_b200_gbam_convert", "rsem_b200_wig_depth", "rsem_b200_gibbs_run_chains", "rsem_b200_gibbs_sum_chains",
+    "rsem_b200_gibbs_split_chains", "rsem_b200_gibbs_upload_from",
 ]
 
 
@@ -164,6 +169,20 @@ class Lib:
         self.check(self.dll.rsem_b200_shard_reads(C.c_uint64(len(row_ptr) - 1), _p(row_ptr, C.c_uint64), C.c_int32(n_shards),
                                                   _p(bounds, C.c_uint64)))
         return [(int(bounds[i]), int(bounds[i + 1])) for i in range(n_shards)]
+
+    def gibbs_split_chains(self, chain_samples, burnin: int, gap: int, n_parts: int):
+        """-> [(first_chain, last_chain_exclusive)] per part: contiguous chain ranges balanced by sweeps"""
+        chain_samples = _arr(chain_samples, np.int32)
+        bounds = np.zeros(n_parts + 1, np.int32)
+        self.check(self.dll.rsem_b200_gibbs_split_chains(C.c_int32(len(chain_samples)), _p(chain_samples, C.c_int32),
+                                                         C.c_int32(burnin), C.c_int32(gap), C.c_int32(n_parts),
+                                                         _p(bounds, C.c_int32)))
+        return [(int(bounds[i]), int(bounds[i + 1])) for i in range(n_parts)]
+
+    def gibbs_sum_chains(self, params: GibbsParams, chain_acc, out: GibbsOut):
+        """out's sums = the params.n_chains per-chain blocks of chain_acc added up in chain order"""
+        chain_acc = _arr(chain_acc, np.float64)
+        self.check(self.dll.rsem_b200_gibbs_sum_chains(C.byref(params), _dp(chain_acc), C.byref(out)))
 
     def comm_unique_id(self) -> bytes:
         buf = C.create_string_buffer(128)
@@ -320,6 +339,20 @@ class Context:
 
     def gibbs_run(self, params: GibbsParams, out: GibbsOut):
         self.lib.check(self.lib.dll.rsem_b200_gibbs_run(self._h, C.byref(params), C.byref(out)))
+
+    def gibbs_run_chains(self, params: GibbsParams, count_vectors: np.ndarray, chain_acc: np.ndarray) -> GibbsStats:
+        """count_vectors: int32 (sum of params.chain_samples) x (M + 1); chain_acc: float64, params.n_chains blocks of
+        4 (M + 1) + n_genes (both C-contiguous, filled in place)"""
+        assert count_vectors.dtype == np.int32 and chain_acc.dtype == np.float64
+        assert count_vectors.flags.c_contiguous and chain_acc.flags.c_contiguous
+        stats = GibbsStats()
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_run_chains(self._h, C.byref(params), _p(count_vectors, C.c_int32),
+                                                               _dp(chain_acc), C.byref(stats)))
+        return stats
+
+    def gibbs_upload_from(self, src: "Context"):
+        """this context gets the matrix uploaded to src (device-to-device copies)"""
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_upload_from(self._h, src._h if src is not None else None))
 
     def sim_begin(self, params: SimParams):
         """params' arrays must stay alive until sim_begin returns (they are copied to the device)"""

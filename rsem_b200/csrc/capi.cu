@@ -1,6 +1,7 @@
 // C ABI glue (include/rsem_b200.h): argument checking, device buffer ownership, stream / NCCL
 // sequencing.  All arithmetic lives in the *_kernels.cu files.
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <algorithm>
 
@@ -711,16 +712,123 @@ int rsem_b200_gibbs_upload(rsem_b200_ctx* c, uint64_t N1, uint64_t E, int32_t M,
     c->gibbs.E = E;
     c->gibbs.M = M;
     if (int rc = gibbs_prepare(c, row_ptr, sid)) return rc;
+    c->gibbs.ready = true;
+    return 0;
+}
+
+int rsem_b200_gibbs_upload_from(rsem_b200_ctx* dst, const rsem_b200_ctx* src) {
+    RB_ARG(dst && src, "NULL argument");
+    RB_ARG(dst != src, "gibbs_upload_from: source and destination are the same context");
+    RB_ARG(src->gibbs.ready, "gibbs_upload_from: the source context holds no completed gibbs_upload");
+    RB_CUDA(cudaSetDevice(dst->device));
+    free_gibbs(dst);
+    if (dst->device != src->device) {   // copies go over NVLink when dst may map src's memory, else through the host
+        int can = 0;
+        RB_CUDA(cudaDeviceCanAccessPeer(&can, dst->device, src->device));
+        if (can) {
+            const cudaError_t e = cudaDeviceEnablePeerAccess(src->device, 0);
+            if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+            else RB_CUDA(e);
+        }
+    }
+    const DevGibbs& s = src->gibbs;
+    DevGibbs& d = dst->gibbs;
+    d.N1 = s.N1; d.E = s.E; d.M = s.M;
+    d.n_comp_tids = s.n_comp_tids; d.n_segs = s.n_segs; d.max_len = s.max_len; d.empty_row = s.empty_row;
+    // same allocation sizes as gibbs_upload / gibbs_prepare; the padding past the data is never copied there either
+    auto copy = [&](auto** to, const auto* from, size_t alloc, size_t n) -> int {
+        if (!from) return 0;
+        RB_CUDA(cudaMalloc(to, alloc * sizeof(**to)));
+        if (n) RB_CUDA(cudaMemcpyPeerAsync(*to, dst->device, from, src->device, n * sizeof(**to), dst->stream));
+        return 0;
+    };
+    int rc = 0;
+    const size_t n_segs = (size_t)s.n_segs;
+    if (!rc) rc = copy(&d.row_ptr, s.row_ptr, s.N1 + 1, s.N1 + 1);
+    if (!rc) rc = copy(&d.sid, s.sid, s.E + 4, s.E);
+    if (!rc) rc = copy(&d.conprb, s.conprb, s.E + 4, s.E);
+    if (!rc) rc = copy(&d.order, s.order, s.N1, s.N1);
+    if (!rc) rc = copy(&d.p_off, s.p_off, s.N1 + 1, s.N1 + 1);
+    if (!rc) rc = copy(&d.p_sid, s.p_sid, s.E + 16, s.E);
+    if (!rc) rc = copy(&d.p_con, s.p_con, s.E + 16, s.E);
+    if (!rc) rc = copy(&d.seg_start, s.seg_start, n_segs + 1, n_segs + 1);
+    if (!rc) rc = copy(&d.seg_ntr, s.seg_ntr, std::max<size_t>(n_segs, 1), n_segs);
+    if (!rc) rc = copy(&d.seg_tid_off, s.seg_tid_off, n_segs + 1, n_segs + 1);
+    if (!rc) rc = copy(&d.comp_tids, s.comp_tids, s.n_comp_tids, s.n_comp_tids);
+    if (!rc) {
+        const cudaError_t e = cudaStreamSynchronize(dst->stream);
+        if (e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    }
+    if (rc) { free_gibbs(dst); return rc; }
+    d.ready = true;
+    return 0;
+}
+
+static int check_gibbs_run(const rsem_b200_ctx* c, const rsem_b200_gibbs_params* p) {
+    RB_ARG(c && p, "NULL argument");
+    RB_ARG(c->gibbs.row_ptr, "gibbs_upload must be called first");
+    RB_ARG(p->M == c->gibbs.M, "M mismatch");
+    RB_ARG(p->n_chains >= 1 && p->chain_samples && p->chain_seeds, "bad chain parameters");
+    return 0;
+}
+
+int rsem_b200_gibbs_run_chains(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
+                               rsem_b200_gibbs_stats* stats) {
+    if (int rc = check_gibbs_run(c, p)) return rc;
+    RB_ARG(count_vectors && chain_acc, "NULL argument");
+    RB_CUDA(cudaSetDevice(c->device));
+    return gibbs_run(c, p, count_vectors, chain_acc, stats);
+}
+
+int rsem_b200_gibbs_sum_chains(const rsem_b200_gibbs_params* p, const double* chain_acc, rsem_b200_gibbs_out* out) {
+    RB_ARG(p && chain_acc && out && out->sum_c && out->sum_c2 && out->sum_tpm && out->sum_fpkm &&
+               (p->n_genes == 0 || out->sum_gene_c2), "NULL argument");
+    RB_ARG(p->M >= 0 && p->n_genes >= 0 && p->n_chains >= 0, "bad sizes");
+    const size_t M1 = (size_t)p->M + 1, acc_per = 4 * M1 + (size_t)p->n_genes;
+    for (size_t i = 0; i < M1; ++i) out->sum_c[i] = out->sum_c2[i] = out->sum_tpm[i] = out->sum_fpkm[i] = 0.0;
+    for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] = 0.0;
+    for (int t = 0; t < p->n_chains; ++t) {   // Gibbs.cpp:372-397: chain 0 first
+        const double* b = chain_acc + (size_t)t * acc_per;
+        for (size_t i = 0; i < M1; ++i) {
+            out->sum_c[i] += b[i];
+            out->sum_c2[i] += b[M1 + i];
+            out->sum_tpm[i] += b[2 * M1 + i];
+            out->sum_fpkm[i] += b[3 * M1 + i];
+        }
+        for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] += b[4 * M1 + gi];
+    }
+    return 0;
+}
+
+int rsem_b200_gibbs_split_chains(int32_t n_chains, const int32_t* chain_samples, int32_t burnin, int32_t gap, int32_t n_parts,
+                                 int32_t* bounds) {
+    RB_ARG(bounds && (n_chains == 0 || chain_samples), "NULL argument");
+    RB_ARG(n_chains >= 0 && n_parts >= 1 && burnin >= 0 && gap >= 1, "bad arguments");
+    std::vector<int64_t> prefix((size_t)n_chains + 1, 0);   // sweeps of chains [0, t)
+    for (int t = 0; t < n_chains; ++t) {
+        RB_ARG(chain_samples[t] >= 1, "every chain keeps at least one sample");
+        prefix[t + 1] = prefix[t] + burnin + 1 + (int64_t)(chain_samples[t] - 1) * gap;
+    }
+    const int used = std::min(n_parts, std::max(n_chains, 1));
+    bounds[0] = 0;
+    for (int i = 1; i < used; ++i) {
+        // nearest to i / used of the total: |used prefix[t] - i total| smallest, the lower t on a tie
+        const int lo = bounds[i - 1] + 1, hi = n_chains - (used - i);
+        int best = lo;
+        for (int t = lo + 1; t <= hi; ++t)
+            if (std::llabs(used * prefix[t] - i * prefix[n_chains]) < std::llabs(used * prefix[best] - i * prefix[n_chains])) best = t;
+        bounds[i] = best;
+    }
+    for (int i = used; i <= n_parts; ++i) bounds[i] = n_chains;
     return 0;
 }
 
 int rsem_b200_gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out) {
-    RB_ARG(c && p && out, "NULL argument");
-    RB_ARG(c->gibbs.row_ptr, "gibbs_upload must be called first");
-    RB_ARG(p->M == c->gibbs.M, "M mismatch");
-    RB_ARG(p->n_chains >= 1 && p->chain_samples && p->chain_seeds, "bad chain parameters");
-    RB_CUDA(cudaSetDevice(c->device));
-    return gibbs_run(c, p, out);
+    RB_ARG(out, "NULL argument");
+    if (int rc = check_gibbs_run(c, p)) return rc;
+    std::vector<double> acc((size_t)p->n_chains * (4 * ((size_t)p->M + 1) + (size_t)std::max(p->n_genes, 0)));
+    if (int rc = rsem_b200_gibbs_run_chains(c, p, out->count_vectors, acc.data(), nullptr)) return rc;
+    return rsem_b200_gibbs_sum_chains(p, acc.data(), out);
 }
 
 int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {

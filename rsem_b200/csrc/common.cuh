@@ -109,9 +109,11 @@ struct DevGibbs {
     int32_t* seg_ntr = nullptr;    // transcripts per component; < 32: rows (p_sid) and assignments hold local ids
     int32_t* seg_tid_off = nullptr;
     int32_t* comp_tids = nullptr;  // sorted transcript ids of every component
+    size_t n_comp_tids = 0;        // entries of comp_tids
     int32_t n_segs = 0;
     uint32_t max_len = 0;
     bool empty_row = false;        // some read has no entry: gibbs_run refuses the matrix before any launch
+    bool ready = false;            // the upload, component layout included, completed (a source for gibbs_upload_from)
 };
 
 // count reduction over NVLink peer memory (p2p.cu)
@@ -328,7 +330,8 @@ int model_launch_conprb(rsem_b200_ctx* ctx);
 int model_launch_update(rsem_b200_ctx* ctx);
 
 // gibbs_kernels.cu
-int gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out);
+int gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
+              rsem_b200_gibbs_stats* stats);
 int gibbs_prepare(rsem_b200_ctx* ctx, const uint64_t* row_ptr, const int32_t* sid);
 
 // sim_kernels.cu

@@ -1137,7 +1137,8 @@ int to_dev(T** d, const T* h, size_t n, cudaStream_t s) {
 
 }  // namespace
 
-static int gibbs_run_serial(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out) {
+static int gibbs_run_serial(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
+                            rsem_b200_gibbs_stats* stats) {
     const DevGibbs& g = c->gibbs;
     const int M1 = p->M + 1, nc = p->n_chains;
     long long total_samples = 0;
@@ -1193,36 +1194,31 @@ static int gibbs_run_serial(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, r
     a.alpha = d_alpha; a.eel = d_eel; a.mw = d_mw; a.gene_start = d_gene; a.counts = d_counts; a.z = d_z;
     a.scratch = d_scratch; a.count_vectors = d_cv; a.acc = d_acc; a.theta_tmp = d_tmp;
 
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    if (stats) { cudaEventCreate(&ev0); cudaEventCreate(&ev1); cudaEventRecord(ev0, c->stream); }
     gibbs_chain_kernel<<<nc, kGibbsThreads, 0, c->stream>>>(a);
     RB_TRYC(cudaGetLastError());
     c->launches++;
+    if (stats) cudaEventRecord(ev1, c->stream);
 
-    std::vector<double> h_acc((size_t)nc * acc_per);
-    RB_TRYC(cudaMemcpyAsync(h_acc.data(), d_acc, h_acc.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaMemcpyAsync(out->count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    RB_TRYC(cudaMemcpyAsync(chain_acc, d_acc, (size_t)nc * acc_per * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    RB_TRYC(cudaMemcpyAsync(count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     int err = 0;
     RB_TRYC(cudaMemcpyAsync(&err, c->err_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     RB_TRYC(cudaStreamSynchronize(c->stream));
     cleanup();
 #undef RB_TRY
 #undef RB_TRYC
+    if (stats) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ev0, ev1);
+        cudaEventDestroy(ev0); cudaEventDestroy(ev1);
+        *stats = rsem_b200_gibbs_stats{ms, 0, 1};
+    }
     if (err) {
         cudaMemset(c->err_flag, 0, sizeof(int));
         set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
         return RSEM_B200_ERR_ARG;
-    }
-    // sum the per-chain accumulators in chain order (Gibbs.cpp:372-397)
-    for (int i = 0; i < M1; ++i) out->sum_c[i] = out->sum_c2[i] = out->sum_tpm[i] = out->sum_fpkm[i] = 0.0;
-    for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] = 0.0;
-    for (int t = 0; t < nc; ++t) {
-        const double* b = h_acc.data() + (size_t)t * acc_per;
-        for (int i = 0; i < M1; ++i) {
-            out->sum_c[i] += b[i];
-            out->sum_c2[i] += b[M1 + i];
-            out->sum_tpm[i] += b[2 * (size_t)M1 + i];
-            out->sum_fpkm[i] += b[3 * (size_t)M1 + i];
-        }
-        for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] += b[4 * (size_t)M1 + gi];
     }
     return 0;
 }
@@ -1350,6 +1346,7 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
     RB_CUDA(cudaMalloc(&g.seg_ntr, std::max<size_t>(seg_ntr.size(), 1) * sizeof(int32_t)));
     RB_CUDA(cudaMalloc(&g.seg_tid_off, seg_tid_off.size() * sizeof(int32_t)));
     RB_CUDA(cudaMalloc(&g.comp_tids, comp_tids.size() * sizeof(int32_t)));
+    g.n_comp_tids = comp_tids.size();
     RB_CUDA(cudaMemcpyAsync(g.seg_ntr, seg_ntr.data(), seg_ntr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     RB_CUDA(cudaMemcpyAsync(g.seg_tid_off, seg_tid_off.data(), seg_tid_off.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     RB_CUDA(cudaMemcpyAsync(g.comp_tids, comp_tids.data(), comp_tids.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
@@ -1357,7 +1354,8 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
     return 0;
 }
 
-static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out) {
+static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
+                              rsem_b200_gibbs_stats* stats) {
     const DevGibbs& g = c->gibbs;
     const int M1 = p->M + 1, nc = p->n_chains;
     long long total_samples = 0;
@@ -1437,7 +1435,8 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
     }
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     const bool timing = getenv("RSEM_B200_TIMING") != nullptr;
-    if (timing) { cudaEventCreate(&ev0); cudaEventCreate(&ev1); cudaEventRecord(ev0, c->stream); }
+    if (timing || stats) { cudaEventCreate(&ev0); cudaEventCreate(&ev1); cudaEventRecord(ev0, c->stream); }
+    int waves = 0;
     for (int base = 0; base < nc; base += chains_per_wave) {
         const int wave = std::min(nc - base, chains_per_wave);
         a.chain_base = base;
@@ -1445,25 +1444,27 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
         void* kargs[] = {(void*)&a};
         RB_TRYC(cudaLaunchCooperativeKernel(kernel, dim3(wave * (ctas + 1)), dim3(kPThreads), kargs, 0, c->stream));
         c->launches++;
+        ++waves;
     }
-    if (timing) cudaEventRecord(ev1, c->stream);
-    std::vector<double> h_acc((size_t)nc * acc_per);
+    if (timing || stats) cudaEventRecord(ev1, c->stream);
     std::vector<ChainSync> h_sync(nc);
-    RB_TRYC(cudaMemcpyAsync(h_acc.data(), d_acc, h_acc.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaMemcpyAsync(out->count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    RB_TRYC(cudaMemcpyAsync(chain_acc, d_acc, (size_t)nc * acc_per * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    RB_TRYC(cudaMemcpyAsync(count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     RB_TRYC(cudaMemcpyAsync(h_sync.data(), d_sync, (size_t)nc * sizeof(ChainSync), cudaMemcpyDeviceToHost, c->stream));
     RB_TRYC(cudaStreamSynchronize(c->stream));
     cleanup();
 #undef RB_TRY
 #undef RB_TRYC
-    if (timing) {
+    if (timing || stats) {
         float ms = 0;
         cudaEventElapsedTime(&ms, ev0, ev1);
         cudaEventDestroy(ev0); cudaEventDestroy(ev1);
+        if (stats) *stats = rsem_b200_gibbs_stats{ms, ctas, waves};
         unsigned max_passes = 0;
         for (int t = 0; t < nc; ++t) max_passes = std::max(max_passes, h_sync[t].passes);
-        fprintf(stderr, "gibbs kernels: %.2f ms on the device (walk variant %d, fast rows %d), most passes of a chain %u\n", ms, pf, a.fast_rows,
-                max_passes);
+        if (timing)
+            fprintf(stderr, "gibbs kernels: %.2f ms on the device (walk variant %d, fast rows %d), most passes of a chain %u\n", ms, pf,
+                    a.fast_rows, max_passes);
     }
     if (timing)
         fprintf(stderr, "gibbs chain 0 (%d worker CTAs, %d segments): %u passes; worker CTA 0 thread 0 cycles: wait for uniforms %llu, passes %llu, "
@@ -1474,29 +1475,18 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
             set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
             return RSEM_B200_ERR_ARG;
         }
-    for (int i = 0; i < M1; ++i) out->sum_c[i] = out->sum_c2[i] = out->sum_tpm[i] = out->sum_fpkm[i] = 0.0;
-    for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] = 0.0;
-    for (int t = 0; t < nc; ++t) {   // per-chain accumulators in chain order (Gibbs.cpp:372-397)
-        const double* b = h_acc.data() + (size_t)t * acc_per;
-        for (int i = 0; i < M1; ++i) {
-            out->sum_c[i] += b[i];
-            out->sum_c2[i] += b[M1 + i];
-            out->sum_tpm[i] += b[2 * (size_t)M1 + i];
-            out->sum_fpkm[i] += b[3 * (size_t)M1 + i];
-        }
-        for (int gi = 0; gi < p->n_genes; ++gi) out->sum_gene_c2[gi] += b[4 * (size_t)M1 + gi];
-    }
     return 0;
 }
 
-int gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_b200_gibbs_out* out) {
+int gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
+              rsem_b200_gibbs_stats* stats) {
     // a row without entries has nothing to draw from (both kernels would fall off its empty cumulative array)
     if (c->gibbs.empty_row) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
     const char* mode = getenv("RSEM_B200_GIBBS");   // "serial" = the one-warp-per-chain kernel (cross-check / debugging)
-    if (mode && !strcmp(mode, "serial")) return gibbs_run_serial(c, p, out);
+    if (mode && !strcmp(mode, "serial")) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
     // tiny inputs: a 624-word regeneration would span more than two sweeps (the generator runs only one sweep ahead)
-    if (c->gibbs.N1 < 1248 || !c->gibbs.order) return gibbs_run_serial(c, p, out);
-    return gibbs_run_parallel(c, p, out);
+    if (c->gibbs.N1 < 1248 || !c->gibbs.order) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
+    return gibbs_run_parallel(c, p, count_vectors, chain_acc, stats);
 }
 
 }  // namespace rsem_b200

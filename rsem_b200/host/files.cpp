@@ -74,6 +74,22 @@ uint32_t parse_seed(const char* s) {
     return seed;
 }
 
+std::vector<int> gpu_devices() {
+    std::vector<int> devices;
+    if (const char* e = getenv("RSEM_B200_DEVICES")) {  // e.g. "0,1,2,3"
+        for (const char* q = e; *q;) {
+            devices.push_back(atoi(q));
+            while (*q && *q != ',') ++q;
+            if (*q == ',') ++q;
+        }
+    }
+    if (devices.size() <= 1) {
+        const char* one = getenv("RSEM_B200_DEVICE");
+        devices.assign(1, one ? atoi(one) : devices.empty() ? 0 : devices[0]);
+    }
+    return devices;
+}
+
 namespace {
 
 struct Cursor {

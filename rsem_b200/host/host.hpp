@@ -323,5 +323,8 @@ std::vector<uint32_t> engine_seeds(uint32_t seed, int n);
 std::vector<char> slurp(const std::string& path, bool must_exist = true);
 void read_type_files(const std::string& imd_name, int tag, int read_type, std::vector<std::string>& files);
 uint32_t parse_seed(const char* s);  // digit-by-digit as EM.cpp:588-593
+// CUDA devices of a multi-GPU run: RSEM_B200_DEVICES=0,1,... in the order given; with at most one entry there,
+// RSEM_B200_DEVICE when it is set, else that entry, else device 0
+std::vector<int> gpu_devices();
 
 }  // namespace host

@@ -266,15 +266,7 @@ int main(int argc, char* argv[]) {
     stamp("reads parsed, initial model estimated");
 
     // ---- device set-up: one worker (host thread + context) per GPU, reads sharded like the reference's threads ----
-    std::vector<int> devices;
-    if (const char* e = getenv("RSEM_B200_DEVICES")) {  // e.g. "0,1,2,3"
-        for (const char* q = e; *q;) {
-            devices.push_back(atoi(q));
-            while (*q && *q != ',') ++q;
-            if (*q == ',') ++q;
-        }
-    }
-    if (devices.size() <= 1) devices.assign(1, env_int("RSEM_B200_DEVICE", devices.empty() ? 0 : devices[0]));
+    std::vector<int> devices = gpu_devices();
     if ((uint64_t)devices.size() > N1) devices.resize((size_t)N1);
     const int world = (int)devices.size();
     std::vector<std::pair<uint64_t, uint64_t>> shards = shard_reads(hits.row_ptr, world);
