@@ -498,11 +498,13 @@ int rsem_b200_set_estep_variant(rsem_b200_ctx* ctx, int32_t variant);
 
 /* Equivalence-class layout the frozen-conprb rounds run on (derived from the hit matrix on first use; reads with
  * identical transcript lists - the reference has no counterpart, it walks HitContainer row by row, EM.cpp:199-244).
- * out[9] = { built (0/1), rows in the layout, rows handled by the long-row launch, segments, batches, tiles,
- *            staged doubles (conprb + ncpv), staged ids, tiles of the main launch }.  Streamed bytes per round =
- *            8 out[6] + 4 out[7] + 16 out[4].  Tiles [0, out[8]) hold the rows of at most 127 hits; the other
- *            out[5] - out[8] tiles (rows of 128..2047 hits) run in a second launch.                                 */
-int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 9 */);
+ * out[10] = { built (0/1), rows in the layout, rows handled by the long-row launch, segments, batches, tiles,
+ *             staged doubles (conprb + ncpv), staged ids, tiles of the main launch, hits in run batches }.  Streamed
+ *             bytes per round = 8 out[6] + 4 out[7] + 16 out[4].  Tiles [0, out[8]) hold the rows of at most 127
+ *             hits; the other out[5] - out[8] tiles (rows of 128..2047 hits) run in a second launch.  A run batch's
+ *             rows hit consecutive transcripts, and it stages one id (the first) per segment, or one per batch when
+ *             all its segments belong to one class, instead of every id.                                          */
+int rsem_b200_class_layout_info(rsem_b200_ctx* ctx, uint64_t* out /* 10 */);
 /* Busy time (ns, %globaltimer) of every persistent CTA in the latest class-layout E-step launch over the main tiles
  * (see rsem_b200_class_layout_info): the evidence for the segmented reduction's load balance on skewed matrices
  * (BASELINE configs[4]).  *n = CTAs written (<= cap); 0 when the layout has no main tiles.                         */

@@ -441,9 +441,9 @@ class Context:
         self.lib.check(self.lib.dll.rsem_b200_set_profiling(self._h, C.c_int32(int(on))))
 
     def class_layout_info(self) -> dict:
-        out = (C.c_uint64 * 9)()
+        out = (C.c_uint64 * 10)()
         self.lib.check(self.lib.dll.rsem_b200_class_layout_info(self._h, out))
-        keys = ("built", "rows", "long_rows", "segments", "batches", "tiles", "vals", "ids", "tiles_main")
+        keys = ("built", "rows", "long_rows", "segments", "batches", "tiles", "vals", "ids", "tiles_main", "run_hits")
         d = dict(zip(keys, (int(x) for x in out)))
         d["bytes_per_round"] = 8 * d["vals"] + 4 * d["ids"] + 16 * d["batches"]
         return d

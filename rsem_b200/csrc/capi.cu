@@ -956,6 +956,7 @@ int rsem_b200_class_layout_info(rsem_b200_ctx* c, uint64_t* out) {
     out[6] = L.n_vals;
     out[7] = L.n_ids;
     out[8] = L.n_tiles_main;
+    out[9] = L.n_run_hits;
     return 0;
 }
 

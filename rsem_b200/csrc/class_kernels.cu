@@ -14,7 +14,8 @@
 //     are stored interleaved (value (segment gi, row r, column c) at (r d + c) nsb + gi) so that every warp-wide
 //     shared-memory load reads 32 consecutive doubles (no bank conflicts), with no padding in HBM;
 //   * ids are stored once per segment (4 B per hit / rows per segment) and row pointers disappear (a batch
-//     descriptor of 16 B replaces them): ~9.2 B per hit at C3 instead of 12.8;
+//     descriptor of 16 B replaces them); a segment over consecutive transcripts (a run, the common case) stores only
+//     its first id: ~8.5 B per hit at C3 instead of 12.8;
 //   * batches are staged by 1-D bulk-async copies (TMA) into a 3-stage shared-memory ring per persistent CTA, as in the
 //     row kernel; each CTA claims tiles from a counter in global memory, no CTA-wide barrier per tile;
 //   * rows longer than kLongDeg hits (never produced behind RSEM's aligner caps of 200) are left out of the
@@ -65,10 +66,21 @@ __host__ __device__ __forceinline__ unsigned rows_cap(unsigned d, unsigned R) {
     return c < 1u ? 1u : (c < R ? c : R);
 }
 
+// A segment is a RUN when its ids are first, first + 1, ..., first + d - 1 (a row over consecutive transcripts: the
+// isoforms of a gene are numbered contiguously).  The ids of a run batch (all its segments runs) are stored as one
+// first per segment, or one for the batch when all its segments belong to one class; other batches store every id.
+// Rows of configuration kTailCfg are never marked runs: the tail launch reads their ids from the stage.
 struct __align__(16) BatchDesc {
     unsigned long long w0;  // val_off (48 bits) | degree << 48
-    unsigned long long w1;  // id_off (40 bits) | rows << 40 | segments << 48 | cfg << 56 | same_class << 60
+    unsigned long long w1;  // id_off (40 bits) | rows << 40 | segments << 48 | cfg << 56 | same_class << 60 | run << 61
 };
+
+// segment sort key: degree << 9 | run << 8 | (255 - rows), 20 bits (degree <= kLongDeg): segments ordered by degree,
+// then non-runs before runs, then by decreasing row count
+constexpr int kKey2Bits = 20;
+__host__ __device__ __forceinline__ unsigned key2_deg(unsigned k) { return k >> 9; }
+__host__ __device__ __forceinline__ unsigned key2_run(unsigned k) { return (k >> 8) & 1u; }
+__host__ __device__ __forceinline__ unsigned key2_rows(unsigned k) { return 255u - (k & 255u); }
 
 struct TileRec {
     unsigned long long val_begin, id_begin, batch_begin;
@@ -197,15 +209,23 @@ __global__ void cls_seg_scatter_kernel(const unsigned long long* __restrict__ ke
     seg_cls[s] = cstart[p];
 }
 
-// key2 = degree << 8 | (255 - rows): segments ordered by degree, then by decreasing row count
-__global__ void cls_seg_key_kernel(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ seg_first,
-                                   unsigned n_segs, unsigned n_rows, unsigned* key2, unsigned* segid) {
+// key2 of every segment (see key2_deg); the rows of a segment share their id list, so its first row decides "run"
+__global__ void cls_seg_key_kernel(const unsigned long long* __restrict__ rp, const int* __restrict__ sid_abs,
+                                   const unsigned long long* __restrict__ keys, const unsigned* __restrict__ rows,
+                                   const unsigned* __restrict__ seg_first, unsigned n_segs, unsigned n_rows, unsigned* key2,
+                                   unsigned* segid) {
     const unsigned s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_segs) return;
     const unsigned first = seg_first[s];
     const unsigned n = (s + 1 < n_segs ? seg_first[s + 1] : n_rows) - first;
     const unsigned d = (unsigned)(keys[first] >> 48);
-    key2[s] = (d << 8) | (255u - n);
+    bool run = d >= 1u && cfg_of_deg(d) != kTailCfg;
+    if (run) {
+        const int* ids = sid_abs + rp[rows[first]];
+        const unsigned id0 = (unsigned)ids[0];
+        for (unsigned c = 1; c < d && run; ++c) run = (unsigned)ids[c] == id0 + c;
+    }
+    key2[s] = (d << 9) | (run ? 256u : 0u) | (255u - n);
     segid[s] = s;
 }
 
@@ -219,7 +239,7 @@ __global__ void cls_batch_flag_kernel(const unsigned* __restrict__ key2s, const 
                                       unsigned n_segs, unsigned* flag) {
     const unsigned f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= n_segs) return;
-    const unsigned P = 32u / group_of_deg(key2s[f] >> 8);
+    const unsigned P = 32u / group_of_deg(key2_deg(key2s[f]));
     flag[f] = ((f - rstart[f]) % P) == 0u ? 1u : 0u;
 }
 
@@ -230,24 +250,28 @@ __global__ void cls_batch_scatter_kernel(const unsigned* __restrict__ flag, cons
     batch_first[bidx1[f] - 1u] = f;
 }
 
-// per batch: value / id counts (scanned into offsets afterwards) and the "all segments belong to one class" flag
+// per batch: value / id counts (scanned into offsets afterwards) and the "all segments belong to one class" flag;
+// *run_hits += the hits of run batches.  A batch's segments share key2, so they are all runs or all not.
 __global__ void cls_batch_size_kernel(const unsigned* __restrict__ key2s, const unsigned* __restrict__ batch_first,
                                       const unsigned* __restrict__ segid_s, const unsigned* __restrict__ seg_cls,
                                       unsigned n_batches, unsigned n_segs, unsigned long long* n_vals,
-                                      unsigned long long* n_ids, unsigned char* same_class, unsigned* max_bytes) {
+                                      unsigned long long* n_ids, unsigned char* same_class, unsigned* max_bytes,
+                                      unsigned long long* run_hits) {
     const unsigned b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= n_batches) return;
     const unsigned f0 = batch_first[b];
     const unsigned nsb = (b + 1 < n_batches ? batch_first[b + 1] : n_segs) - f0;
-    const unsigned k = key2s[f0], d = k >> 8, n = 255u - (k & 255u);
+    const unsigned k = key2s[f0], d = key2_deg(k), n = key2_rows(k);
+    const unsigned per_seg = key2_run(k) ? 1u : d;  // ids stored per segment
     const unsigned long long nv = (unsigned long long)nsb * n * (d + 1u);
     bool same = true;
     const unsigned c0 = seg_cls[segid_s[f0]];
     for (unsigned i = 1; i < nsb; ++i) same = same && seg_cls[segid_s[f0 + i]] == c0;
     n_vals[b] = nv;
     same_class[b] = same ? 1 : 0;
-    n_ids[b] = same ? d : (unsigned long long)nsb * d;
-    atomicMax(max_bytes, (unsigned)(8u * nv + 4u * nsb * d + 16u));
+    n_ids[b] = same ? per_seg : (unsigned long long)nsb * per_seg;
+    atomicMax(max_bytes, (unsigned)(8u * nv + 4u * nsb * per_seg + 16u));
+    if (key2_run(k)) atomicAdd(run_hits, (unsigned long long)nsb * n * d);
 }
 
 __global__ void cls_batch_desc_kernel(const unsigned* __restrict__ key2s, const unsigned* __restrict__ batch_first,
@@ -259,11 +283,12 @@ __global__ void cls_batch_desc_kernel(const unsigned* __restrict__ key2s, const 
     if (b >= n_batches) return;
     const unsigned f0 = batch_first[b];
     const unsigned nsb = (b + 1 < n_batches ? batch_first[b + 1] : n_segs) - f0;
-    const unsigned k = key2s[f0], d = k >> 8, n = 255u - (k & 255u);
+    const unsigned k = key2s[f0], d = key2_deg(k), n = key2_rows(k);
     BatchDesc o;
     o.w0 = val_off[b] | ((unsigned long long)d << 48);
     o.w1 = id_off[b] | ((unsigned long long)n << 40) | ((unsigned long long)nsb << 48) |
-           ((unsigned long long)cfg_of_deg(d) << 56) | ((unsigned long long)same_class[b] << 60);
+           ((unsigned long long)cfg_of_deg(d) << 56) | ((unsigned long long)same_class[b] << 60) |
+           ((unsigned long long)key2_run(k) << 61);
     desc[b] = o;
 }
 
@@ -280,7 +305,7 @@ __global__ void cls_tail_start_kernel(const unsigned* __restrict__ key2s, const 
     unsigned lo = 0, hi = n_batches;
     while (lo < hi) {
         const unsigned mid = (lo + hi) >> 1;
-        if (cfg_of_deg(key2s[batch_first[mid]] >> 8) != kTailCfg) lo = mid + 1;
+        if (cfg_of_deg(key2_deg(key2s[batch_first[mid]])) != kTailCfg) lo = mid + 1;
         else hi = mid;
     }
     out[0] = lo;
@@ -316,7 +341,8 @@ __global__ void cls_tile_rec_kernel(const unsigned long long* __restrict__ bound
     rec[k].batch_begin = b;
 }
 
-// one warp per batch: ids of segment gi, column c at id_off + c nsb + gi (or id_off + c for a one-class batch)
+// one warp per batch: ids of segment gi, column c at id_off + c nsb + gi (or id_off + c for a one-class batch); a run
+// batch stores column 0 only (the segments' firsts)
 __global__ void cls_fill_ids_kernel(const unsigned long long* __restrict__ rp, const int* __restrict__ sid_abs,
                                     const BatchDesc* __restrict__ desc, const unsigned* __restrict__ batch_first,
                                     const unsigned* __restrict__ fseg_first, const unsigned* __restrict__ rows,
@@ -325,7 +351,8 @@ __global__ void cls_fill_ids_kernel(const unsigned long long* __restrict__ rp, c
     for (unsigned long long b = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n_batches;
          b += ((unsigned long long)gridDim.x * blockDim.x) >> 5) {
         const BatchDesc bd = desc[b];
-        const unsigned d = (unsigned)(bd.w0 >> 48), nsb = (unsigned)(bd.w1 >> 48) & 255u, same = (unsigned)(bd.w1 >> 60) & 1u;
+        const unsigned nsb = (unsigned)(bd.w1 >> 48) & 255u, same = (unsigned)(bd.w1 >> 60) & 1u;
+        const unsigned d = (bd.w1 >> 61) & 1u ? 1u : (unsigned)(bd.w0 >> 48);  // ids stored per segment
         const unsigned long long ioff = bd.w1 & kOff40;
         const unsigned f0 = batch_first[b];
         const unsigned ns = same ? 1u : nsb;
@@ -527,17 +554,19 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
 // gi: ids and theta are loaded once, the rows are walked U at a time (instruction-level parallelism across the
 // load -> product -> row sum -> reciprocal chain), the normalised weights are summed per lane and leave as ONE
 // reduction per transcript and segment.  The noise column's sum stays in the thread (count[0] is flushed per CTA).
+// run: the batch stores its segments' firsts, column c < d is transcript first + c.
 // PROF: ph[] takes the cycles from t0 (read by the caller before it loaded the batch's descriptor) to theta usable,
 // of the row walk and of the flush.
 template <int G, int S, int U, bool TAIL, bool PROF>
 __device__ __forceinline__ double process_batch(const double* __restrict__ bv, const int* __restrict__ bi, unsigned d,
-                                                unsigned n, unsigned nsb, bool same, const double* __restrict__ theta,
+                                                unsigned n, unsigned nsb, bool same, bool run, const double* __restrict__ theta,
                                                 double* count, unsigned lane, long long t0, long long (&ph)[kPhases]) {
     constexpr unsigned P = 32 / G;
     const unsigned gi = lane % P, g = lane / P;
     const bool seg_ok = gi < nsb;
     const unsigned w = d + 1u;
     const unsigned ids_stride = same ? 1u : nsb, ids_gi = same ? 0u : gi;
+    const int first = (run && seg_ok) ? bi[ids_gi] : 0;
     int t[S];
     double th[S], acc[S];
     bool col_ok[S];
@@ -547,7 +576,8 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
         const unsigned c = g + G * q;
         col_ok[q] = seg_ok && c < w;
         coff[q] = c * nsb;
-        t[q] = (seg_ok && c < d) ? bi[c * ids_stride + ids_gi] : 0;  // column d is the noise entry: transcript 0
+        // column d is the noise entry: transcript 0
+        t[q] = (seg_ok && c < d) ? (run ? first + (int)c : bi[c * ids_stride + ids_gi]) : 0;
     }
 #pragma unroll
     for (int q = 0; q < S; ++q) {
@@ -670,7 +700,7 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
                 const BatchDesc bd = s_desc[b];
                 const unsigned d = (unsigned)(bd.w0 >> 48), n = (unsigned)(bd.w1 >> 40) & 255u, nsb = (unsigned)(bd.w1 >> 48) & 255u;
                 const unsigned cfg = (unsigned)(bd.w1 >> 56) & 15u;
-                const bool same = (bd.w1 >> 60) & 1ull;
+                const bool same = (bd.w1 >> 60) & 1ull, run = (bd.w1 >> 61) & 1ull;
                 const double* bv = s_val + ((bd.w0 & kOff48) - sd.val_base);
                 const int* bi = s_ids + ((bd.w1 & kOff40) - sd.id_base);
 #ifdef RB_CLASS_DEBUG
@@ -690,21 +720,21 @@ __global__ void __launch_bounds__((W + 1) * 32, 1) estep_class_kernel(const Clas
                 }
 #endif
                 if constexpr (TAIL) {
-                    acc0 += process_batch<32, 4, U, true, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph);
+                    acc0 += process_batch<32, 4, U, true, PROF>(bv, bi, d, n, nsb, same, false, a.theta, a.count, lane, tc, ph);
                 } else {
                     switch (cfg) {
-                        case 0: acc0 += process_batch<1, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 1: acc0 += process_batch<1, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 2: acc0 += process_batch<2, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 3: acc0 += process_batch<2, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 4: acc0 += process_batch<4, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 5: acc0 += process_batch<4, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 6: acc0 += process_batch<8, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 7: acc0 += process_batch<8, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 8: acc0 += process_batch<16, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 9: acc0 += process_batch<16, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        case 10: acc0 += process_batch<32, 3, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
-                        default: acc0 += process_batch<32, 4, U, false, PROF>(bv, bi, d, n, nsb, same, a.theta, a.count, lane, tc, ph); break;
+                        case 0: acc0 += process_batch<1, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 1: acc0 += process_batch<1, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 2: acc0 += process_batch<2, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 3: acc0 += process_batch<2, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 4: acc0 += process_batch<4, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 5: acc0 += process_batch<4, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 6: acc0 += process_batch<8, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 7: acc0 += process_batch<8, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 8: acc0 += process_batch<16, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 9: acc0 += process_batch<16, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        case 10: acc0 += process_batch<32, 3, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
+                        default: acc0 += process_batch<32, 4, U, false, PROF>(bv, bi, d, n, nsb, same, run, a.theta, a.count, lane, tc, ph); break;
                     }
                 }
             }
@@ -944,18 +974,18 @@ int class_build(rsem_b200_ctx* ctx) {
     RB_CUDA(sc.alloc(&key2_s, n_segs));
     RB_CUDA(sc.alloc(&segid, n_segs));
     RB_CUDA(sc.alloc(&segid_s, n_segs));
-    cls_seg_key_kernel<<<blocks_for(n_segs, 256), 256, 0, st>>>(keys_s, seg_first, n_segs, n_rows, key2, segid);
+    cls_seg_key_kernel<<<blocks_for(n_segs, 256), 256, 0, st>>>(rp, sid_abs, keys_s, rows_s, seg_first, n_segs, n_rows, key2, segid);
     RB_CUDA(cudaGetLastError());
     {
         size_t need2 = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, need2, key2, key2_s, segid, segid_s, (long long)n_segs, 0, 20, st);
+        cub::DeviceRadixSort::SortPairs(nullptr, need2, key2, key2_s, segid, segid_s, (long long)n_segs, 0, kKey2Bits, st);
         if (need2 > tmp_bytes) {
             sc.release(tmp);
             RB_CUDA(sc.alloc(reinterpret_cast<unsigned char**>(&tmp), need2));
             tmp_bytes = need2;
         }
         need2 = tmp_bytes;
-        RB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, need2, key2, key2_s, segid, segid_s, (long long)n_segs, 0, 20, st));
+        RB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, need2, key2, key2_s, segid, segid_s, (long long)n_segs, 0, kKey2Bits, st));
     }
     RB_CUDA(cudaStreamSynchronize(st));
     sc.release(keys_s); keys_s = nullptr;
@@ -976,7 +1006,10 @@ int class_build(rsem_b200_ctx* ctx) {
     cls_batch_scatter_kernel<<<blocks_for(n_segs, 256), 256, 0, st>>>(s_a, s_c, n_segs, L.batch_first);
     RB_CUDA(cudaGetLastError());
     unsigned long long *n_vals = nullptr, *n_ids = nullptr, *val_off = nullptr, *id_off = nullptr;
+    unsigned long long* run_hits = nullptr;
     unsigned char* same_class = nullptr;
+    RB_CUDA(sc.alloc(&run_hits, 1));
+    RB_CUDA(cudaMemsetAsync(run_hits, 0, sizeof(unsigned long long), st));
     RB_CUDA(sc.alloc(&n_vals, (size_t)n_batches + 1));
     RB_CUDA(sc.alloc(&n_ids, (size_t)n_batches + 1));
     RB_CUDA(sc.alloc(&val_off, (size_t)n_batches + 1));
@@ -985,15 +1018,16 @@ int class_build(rsem_b200_ctx* ctx) {
     RB_CUDA(cudaMemsetAsync(n_vals + n_batches, 0, sizeof(unsigned long long), st));
     RB_CUDA(cudaMemsetAsync(n_ids + n_batches, 0, sizeof(unsigned long long), st));
     cls_batch_size_kernel<<<blocks_for(n_batches, 256), 256, 0, st>>>(key2_s, L.batch_first, segid_s, seg_cls, n_batches, n_segs,
-                                                                     n_vals, n_ids, same_class, d_cnt + 1);
+                                                                     n_vals, n_ids, same_class, d_cnt + 1, run_hits);
     RB_CUDA(cudaGetLastError());
     need = tmp_bytes;
     RB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, need, n_vals, val_off, (long long)n_batches + 1, st));
     need = tmp_bytes;
     RB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, need, n_ids, id_off, (long long)n_batches + 1, st));
-    unsigned long long totals[2] = {0, 0};
+    unsigned long long totals[3] = {0, 0, 0};
     RB_CUDA(cudaMemcpyAsync(&totals[0], val_off + n_batches, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     RB_CUDA(cudaMemcpyAsync(&totals[1], id_off + n_batches, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    RB_CUDA(cudaMemcpyAsync(&totals[2], run_hits, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     RB_CUDA(cudaMemcpyAsync(h_cnt, d_cnt, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     RB_CUDA(cudaStreamSynchronize(st));
     const unsigned max_batch_bytes = h_cnt[1];
@@ -1004,6 +1038,7 @@ int class_build(rsem_b200_ctx* ctx) {
     pt.mark("segments sorted, batches formed");
     L.n_vals = totals[0];
     L.n_ids = totals[1];
+    L.n_run_hits = totals[2];
     L.n_segs = n_segs;
     L.n_batches = n_batches;
     RB_CUDA(block_alloc(ctx, reinterpret_cast<void**>(&L.desc), ((size_t)n_batches + 1) * sizeof(BatchDesc)));
@@ -1136,8 +1171,16 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         //   C2                      0.373  0.373  0.376  0.371  0.372  0.374  0.372  0.372  0.374  0.370  0.371  0.405
         //   C5                      8.167  8.292  8.589  7.952  8.044  8.294  7.813  7.977  8.187  7.818  7.895  8.302
         // (18 x 3 and 18 x 4 spill; the sweep predates the evict_first priority of the copies, which took 15 x 2 at C3
-        // from 3.39 to 3.20 ms and has not been swept.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
+        // from 3.39 to 3.20 ms.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
         // registers), in a separate process on the same card: C3 3.519, C2 0.373, C5 8.579.
+        // Re-swept with evict_first and run batches (same card, one process per run, 3 alternating runs, ms per round):
+        //   consumer warps x rows:  14x2                 15x2                 18x2
+        //   C3                      3.039 3.040 3.036    3.028 3.041 3.029    3.030 3.031 3.032
+        //   C2                      0.357 0.356 0.352    0.353 0.360 0.351    0.356 0.353 0.354
+        //   C5                      7.561 7.562 7.540    7.428 7.421 7.398    7.216 7.213 7.202
+        // 18 warps tie at C3 and C2 and are 2.7 % faster at C5 (88 registers), but their profiling instantiation
+        // spills (16 bytes), so 15 stays: the profiled launch (tools/k2_anatomy.py) has to run the configuration
+        // that is timed, or its phase shares describe another kernel, and no instantiation may spill.
         constexpr int W = 15, U = 2;
         const size_t smem = sizeof(ClassSmem<W>);
         if (ctx->profiling) {

@@ -138,8 +138,10 @@ struct ClassLayout {
     uint32_t n_rows = 0, n_long = 0, n_segs = 0, n_batches = 0, n_tiles = 0, R = 0;
     uint32_t n_tiles_main = 0;      // tiles [0, n_tiles_main): rows of <= 127 hits; the rest: longer rows (own launch)
     uint64_t n_vals = 0, n_ids = 0;
+    uint64_t n_run_hits = 0;        // hits in batches whose segments hit consecutive transcripts (ids stored as firsts)
     double* vals = nullptr;         // per batch: ncpv [row][segment], then conprb [(row, column)][segment]
-    int32_t* ids = nullptr;         // per batch: transcript ids [column][segment] (or [column] for a one-class batch)
+    int32_t* ids = nullptr;         // per batch: transcript ids [column][segment] (or [column] for a one-class batch);
+                                    // a run batch: first id [segment] (or one for a one-class batch)
     void* desc = nullptr;           // BatchDesc[n_batches]
     void* tile = nullptr;           // TileRec[n_tiles + 1]
     uint32_t* batch_first = nullptr;  // first segment (final order) of every batch
