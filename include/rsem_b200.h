@@ -37,6 +37,9 @@ extern "C" {
 #define RSEM_B200_ERR_ARG 2      /* invalid argument / call order */
 #define RSEM_B200_ERR_NCCL 3     /* NCCL failure or libnccl not loadable */
 #define RSEM_B200_ERR_UNSUPPORTED 4
+#define RSEM_B200_ERR_FULL 5       /* rsem_b200_batch_add: the sample does not fit the arena's remaining bytes */
+
+typedef struct rsem_b200_batch rsem_b200_batch;
 
 typedef struct rsem_b200_ctx rsem_b200_ctx;
 
@@ -484,6 +487,48 @@ int rsem_b200_wig_depth(rsem_b200_ctx* ctx, const rsem_b200_wig_batch* batch, do
 
 /* ---- instrumentation (bench / tests) ----------------------------------------------------------- */
 /* number of kernels this library launched on ctx since creation */
+/* ---- K12: frozen-conprb rounds of many samples at once (rsem-run-em-batch) --------------------------------------
+ * A batch holds the frozen matrices (conprb, ncpv of ROUND >= 11) of several samples in one device arena and runs their
+ * rounds of EM.cpp:364-416 (E_STEP EM.cpp:199-244, M-step EM.cpp:385-398, bChange / totNum EM.cpp:406-413, stop test
+ * EM.cpp:416) in one kernel: a CTA owns a sample and runs its rounds back to back.  Each sample is kept in the space
+ * of the transcripts its hits name; this is exact from round 2 on, where theta is 0 for every other transcript.
+ * The batch lives on `ctx`'s device and stream; destroy it before the context.                                      */
+
+/* capacity_bytes = 0: half of the device memory free at the call. */
+int rsem_b200_batch_create(rsem_b200_ctx* ctx, uint64_t capacity_bytes, rsem_b200_batch** out);
+int rsem_b200_batch_destroy(rsem_b200_batch* batch);
+
+/* Device bytes a sample of this shape takes in an arena (m = its number of distinct transcripts), or
+ * RSEM_B200_ERR_UNSUPPORTED when it is outside the batch layout (more than 2^20 hits, more than 12287 distinct
+ * transcripts, or a read with more than 2048 alignments): such a sample runs with rsem_b200_em_rounds.  No GPU needed. */
+int rsem_b200_batch_sample_bytes(uint64_t N, uint64_t H, const uint64_t* row_ptr, int32_t m, uint64_t* bytes);
+
+/* Adds a sample whose next round is `first_round` (>= 2): its CSR matrix (row_ptr N + 1, sid H, signed as in the .dat),
+ * frozen conprb (H) / ncpv (N), theta (M + 1) after round first_round - 1 and N0.  Refused with RSEM_B200_ERR_ARG when
+ * theta is not exactly 0 for a transcript no hit names, RSEM_B200_ERR_FULL when the arena has no room left for it,
+ * RSEM_B200_ERR_UNSUPPORTED as rsem_b200_batch_sample_bytes.  *slot receives its handle.                            */
+int rsem_b200_batch_add(rsem_b200_batch* batch, uint64_t N, uint64_t H, int32_t M, const uint64_t* row_ptr,
+                        const int32_t* sid, const double* conprb, const double* ncpv, const double* theta, double n0,
+                        int32_t first_round, int32_t min_round, int32_t max_round, int32_t* slot);
+
+/* One launch: every sample that has not stopped runs up to `max_rounds` rounds.  Arrays are indexed by slot and sized
+ * by rsem_b200_batch_slots: stats (slots x max_rounds, may be NULL) receives each round's (sum, bChange, totNum) of
+ * the "ROUND = ..." line (EM.cpp:415), rounds_run the number of rounds the slot ran, stopped 1 once the slot's loop
+ * condition ROUND < min_round || (totNum > 0 && ROUND < max_round) became false.                                   */
+int rsem_b200_batch_run(rsem_b200_batch* batch, int32_t max_rounds, rsem_b200_round_stats* stats, int32_t* rounds_run,
+                        int32_t* stopped);
+int rsem_b200_batch_slots(rsem_b200_batch* batch, int32_t* n_slots);
+
+/* Final pass with calcExpectedWeights = true (EM.cpp:460-478) for one sample: theta (M + 1) and the expected counts
+ * (M + 1, WITHOUT N0) scattered back to transcript ids, and when not NULL the posteriors per hit (H) and of the noise
+ * entry per read (N), as rsem_b200_expected_weights gives them.  theta is not changed; the sample stays in the batch. */
+int rsem_b200_batch_final(rsem_b200_batch* batch, int32_t slot, double* theta, double* counts, double* post,
+                          double* post0);
+/* Frees a sample's bytes in the arena. */
+int rsem_b200_batch_remove(rsem_b200_batch* batch, int32_t slot);
+/* K12 device time summed over launches (CUDA events) and the sample-rounds they ran. */
+int rsem_b200_batch_timing(rsem_b200_batch* batch, double* total_ms, uint64_t* sample_rounds);
+
 int rsem_b200_launch_count(rsem_b200_ctx* ctx, uint64_t* launches);
 /* device time (ms, CUDA events on the context's stream) spent in the E/M kernel (K2) launches and
  * their number since the last reset; used for the roofline figure.                              */

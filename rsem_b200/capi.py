@@ -135,8 +135,12 @@ SYMBOLS = [
     "rsem_b200_estep_cta_times", "rsem_b200_estep_wait_times", "rsem_b200_sim_begin", "rsem_b200_sim_next",
     "rsem_b200_sim_end", "rsem_b200_ci_begin", "rsem_b200_ci_push", "rsem_b200_ci_end", "rsem_b200_kmer_shared",
     "rsem_b200_gbam_convert", "rsem_b200_wig_depth", "rsem_b200_gibbs_run_chains", "rsem_b200_gibbs_sum_chains",
-    "rsem_b200_gibbs_split_chains", "rsem_b200_gibbs_upload_from",
+    "rsem_b200_gibbs_split_chains", "rsem_b200_gibbs_upload_from", "rsem_b200_batch_create", "rsem_b200_batch_destroy",
+    "rsem_b200_batch_sample_bytes", "rsem_b200_batch_add", "rsem_b200_batch_run", "rsem_b200_batch_slots",
+    "rsem_b200_batch_final", "rsem_b200_batch_remove", "rsem_b200_batch_timing",
 ]
+
+RSEM_B200_ERR_FULL = 5
 
 
 class Lib:
@@ -465,3 +469,83 @@ class Context:
 
     def set_estep_variant(self, v: int):
         self.lib.check(self.lib.dll.rsem_b200_set_estep_variant(self._h, C.c_int32(v)))
+
+
+class Batch:
+    """K12: the frozen-conprb rounds of many samples in one device arena (include/rsem_b200.h, rsem_b200_batch_*)."""
+
+    def __init__(self, ctx: Context, capacity_bytes: int = 0):
+        self.lib = ctx.lib
+        self.ctx = ctx   # the batch lives on the context's device and stream
+        self._h = C.c_void_p()
+        self.lib.check(self.lib.dll.rsem_b200_batch_create(ctx._h, C.c_uint64(capacity_bytes), C.byref(self._h)))
+        self.shapes = {}
+
+    def close(self):
+        if self._h:
+            self.lib.dll.rsem_b200_batch_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def sample_bytes(self, row_ptr, m: int) -> int:
+        row_ptr = _arr(row_ptr, np.uint64)
+        out = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rsem_b200_batch_sample_bytes(
+            C.c_uint64(len(row_ptr) - 1), C.c_uint64(int(row_ptr[-1])), _p(row_ptr, C.c_uint64), C.c_int32(m),
+            C.byref(out)))
+        return out.value
+
+    def add(self, row_ptr, sid, conprb, ncpv, theta, n0: float, first_round: int, min_round: int, max_round: int) -> int:
+        """returns the slot; raises RsemB200Error (code RSEM_B200_ERR_FULL in .code) when the arena is full"""
+        row_ptr, sid = _arr(row_ptr, np.uint64), _arr(sid, np.int32)
+        conprb, ncpv, theta = _arr(conprb, np.float64), _arr(ncpv, np.float64), _arr(theta, np.float64)
+        N, H, M = len(row_ptr) - 1, len(sid), len(theta) - 1
+        slot = C.c_int32(-1)
+        rc = self.lib.dll.rsem_b200_batch_add(
+            self._h, C.c_uint64(N), C.c_uint64(H), C.c_int32(M), _p(row_ptr, C.c_uint64), _p(sid, C.c_int32),
+            _dp(conprb), _dp(ncpv), _dp(theta), C.c_double(n0), C.c_int32(first_round), C.c_int32(min_round),
+            C.c_int32(max_round), C.byref(slot))
+        if rc != 0:
+            err = RsemB200Error(f"librsem_b200 error {rc}: {self.lib.dll.rsem_b200_last_error().decode()}")
+            err.code = rc
+            raise err
+        self.shapes[slot.value] = (N, H, M)
+        return slot.value
+
+    def run(self, max_rounds: int):
+        """one launch; returns {slot: (list of (sum, bchange, totnum), stopped)}"""
+        n = C.c_int32(0)
+        self.lib.check(self.lib.dll.rsem_b200_batch_slots(self._h, C.byref(n)))
+        k = max(max_rounds, 1)
+        stats = (RoundStats * (max(n.value, 1) * k))()
+        ran = np.zeros(max(n.value, 1), np.int32)
+        stopped = np.zeros(max(n.value, 1), np.int32)
+        self.lib.check(self.lib.dll.rsem_b200_batch_run(self._h, C.c_int32(max_rounds), stats, _p(ran, C.c_int32),
+                                                        _p(stopped, C.c_int32)))
+        return {s: ([(stats[s * k + r].sum, stats[s * k + r].bchange, stats[s * k + r].totnum) for r in range(ran[s])],
+                    bool(stopped[s])) for s in self.shapes}
+
+    def final(self, slot: int, posteriors: bool = False):
+        """(theta M + 1, counts M + 1 without N0, post H or None, post0 N or None)"""
+        N, H, M = self.shapes[slot]
+        theta, counts = np.empty(M + 1), np.empty(M + 1)
+        post = np.empty(max(H, 1)) if posteriors else None
+        post0 = np.empty(N) if posteriors else None
+        self.lib.check(self.lib.dll.rsem_b200_batch_final(self._h, C.c_int32(slot), _dp(theta), _dp(counts), _dp(post),
+                                                          _dp(post0)))
+        return theta, counts, (post[:H] if posteriors else None), post0
+
+    def remove(self, slot: int):
+        self.lib.check(self.lib.dll.rsem_b200_batch_remove(self._h, C.c_int32(slot)))
+        del self.shapes[slot]
+
+    def timing(self):
+        """(K12 device ms summed over launches, sample-rounds run)"""
+        ms, n = C.c_double(0), C.c_uint64(0)
+        self.lib.check(self.lib.dll.rsem_b200_batch_timing(self._h, C.byref(ms), C.byref(n)))
+        return ms.value, n.value

@@ -924,6 +924,64 @@ int rsem_b200_wig_depth(rsem_b200_ctx* c, const rsem_b200_wig_batch* b, double* 
     return wig_depth(c, b, out, out_cap, out_len, stats);
 }
 
+int rsem_b200_batch_create(rsem_b200_ctx* c, uint64_t capacity_bytes, rsem_b200_batch** out) {
+    RB_ARG(c && out, "NULL argument");
+    return batch_create(c, capacity_bytes, out);
+}
+
+int rsem_b200_batch_destroy(rsem_b200_batch* b) {
+    if (b) batch_destroy(b);
+    return 0;
+}
+
+int rsem_b200_batch_sample_bytes(uint64_t N, uint64_t H, const uint64_t* row_ptr, int32_t m, uint64_t* bytes) {
+    RB_ARG(row_ptr && bytes, "NULL argument");
+    RB_ARG(m >= 0 && row_ptr[0] == 0 && row_ptr[N] == H, "row_ptr must start at 0 and end at H, m >= 0");
+    return batch_sample_bytes(N, H, row_ptr, m, bytes);
+}
+
+int rsem_b200_batch_add(rsem_b200_batch* b, uint64_t N, uint64_t H, int32_t M, const uint64_t* row_ptr,
+                        const int32_t* sid, const double* conprb, const double* ncpv, const double* theta, double n0,
+                        int32_t first_round, int32_t min_round, int32_t max_round, int32_t* slot) {
+    RB_ARG(b && row_ptr && (sid || H == 0) && (conprb || H == 0) && (ncpv || N == 0) && theta && slot, "NULL argument");
+    RB_ARG(M >= 1 && N >= 1, "M and N must be >= 1");
+    RB_ARG(row_ptr[0] == 0 && row_ptr[N] == H, "row_ptr must start at 0 and end at H");
+    for (uint64_t i = 0; i < N; ++i) RB_ARG(row_ptr[i] <= row_ptr[i + 1], "row_ptr must not decrease");
+    RB_ARG(first_round >= 2, "the batch starts after round 1 (first_round >= 2)");
+    return batch_add(b, N, H, M, row_ptr, sid, conprb, ncpv, theta, n0, first_round, min_round, max_round, slot);
+}
+
+int rsem_b200_batch_run(rsem_b200_batch* b, int32_t max_rounds, rsem_b200_round_stats* stats, int32_t* rounds_run,
+                        int32_t* stopped) {
+    RB_ARG(b && rounds_run && stopped, "NULL argument");
+    RB_ARG(max_rounds >= 0, "max_rounds < 0");
+    return batch_run(b, max_rounds, stats, rounds_run, stopped);
+}
+
+int rsem_b200_batch_slots(rsem_b200_batch* b, int32_t* n_slots) {
+    RB_ARG(b && n_slots, "NULL argument");
+    *n_slots = batch_slots(b);
+    return 0;
+}
+
+int rsem_b200_batch_final(rsem_b200_batch* b, int32_t slot, double* theta, double* counts, double* post, double* post0) {
+    RB_ARG(b, "NULL argument");
+    RB_ARG(batch_slot_live(b, slot), "no sample in this slot");
+    return batch_final(b, slot, theta, counts, post, post0);
+}
+
+int rsem_b200_batch_remove(rsem_b200_batch* b, int32_t slot) {
+    RB_ARG(b, "NULL argument");
+    RB_ARG(batch_slot_live(b, slot), "no sample in this slot");
+    batch_remove(b, slot);
+    return 0;
+}
+
+int rsem_b200_batch_timing(rsem_b200_batch* b, double* total_ms, uint64_t* sample_rounds) {
+    RB_ARG(b && total_ms && sample_rounds, "NULL argument");
+    return batch_timing(b, total_ms, sample_rounds);
+}
+
 int rsem_b200_launch_count(rsem_b200_ctx* c, uint64_t* launches) {
     RB_ARG(c && launches, "NULL argument");
     *launches = c->launches;

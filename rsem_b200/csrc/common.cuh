@@ -187,7 +187,21 @@ __device__ __forceinline__ int aux_len(const uint8_t* s, const uint8_t* end) {
 struct SimState;  // sim_kernels.cu
 struct CiState;   // ci_kernels.cu
 struct GbamState; // gbam_kernels.cu
-struct WigState;  // wiggle_kernels.cu
+struct WigState;  // batch_kernels.cu
+int batch_create(rsem_b200_ctx* ctx, uint64_t capacity, rsem_b200_batch** out);
+void batch_destroy(rsem_b200_batch* b);
+int batch_sample_bytes(uint64_t N, uint64_t H, const uint64_t* row_ptr, int32_t m, uint64_t* bytes);
+int batch_add(rsem_b200_batch* b, uint64_t N, uint64_t H, int32_t M, const uint64_t* row_ptr, const int32_t* sid,
+              const double* conprb, const double* ncpv, const double* theta, double n0, int32_t first_round,
+              int32_t min_round, int32_t max_round, int32_t* slot);
+int batch_run(rsem_b200_batch* b, int32_t rounds, rsem_b200_round_stats* stats, int32_t* rounds_run, int32_t* stopped);
+int batch_final(rsem_b200_batch* b, int32_t slot, double* theta, double* counts, double* post, double* post0);
+void batch_remove(rsem_b200_batch* b, int slot);
+int batch_slots(const rsem_b200_batch* b);
+bool batch_slot_live(const rsem_b200_batch* b, int slot);
+int batch_timing(const rsem_b200_batch* b, double* ms, uint64_t* sample_rounds);
+
+// wiggle_kernels.cu
 
 }  // namespace rsem_b200
 

@@ -185,6 +185,10 @@ void expression_values(const std::vector<double>& theta, const std::vector<doubl
 void write_results_em(const std::string& ref_name, const std::string& imd_name, const std::vector<TranscriptInfo>& tr,
                       const std::vector<double>& theta, const std::vector<double>& eel, const double* counts,
                       bool append_names);  // WriteResults.h:125-355
+// em_sample.cpp: the per-sample output stages of rsem-run-em (also used by rsem-run-em-batch)
+void write_em_outputs(const std::string& refName, const std::string& imdName, const std::string& statName,
+                      const RefData& refs, const std::vector<TranscriptInfo>& transcripts, const HostModel& model,
+                      std::vector<double> theta, const std::vector<double>& counts, bool appendNames);
 void write_results_gibbs(const std::string& ref_name, const std::string& imd_name, int M, const std::vector<double>& pme_c,
                          const std::vector<double>& pme_fpkm, const std::vector<double>& pme_tpm,
                          const std::vector<double>& pve_c, const std::vector<double>& pve_c_genes,
@@ -316,6 +320,12 @@ struct Mt {
     }
     double uniform01() { return next() * (1.0 / 4294967296.0); }  // boost uniform_01 on a 32-bit engine
 };
+
+// em_sample.cpp: sampleName.transcript.bam with the posteriors of the final pass (EM.cpp:504-536, BamWriter.h)
+void write_posterior_bam(const std::string& inpSamF, const std::string& outName, int read_type, bool sampling, bool hasSeed,
+                         uint32_t seed, const std::vector<TranscriptInfo>& tr, int ti_type, const HitStore& hits,
+                         std::vector<double>& post, const std::vector<double>& post0, int threads, bool verbose);
+
 
 // ---- small utilities -----------------------------------------------------------------------------
 // engineFactory (sampling.h:19-40): n engine seeds drawn from mt19937(seed), a seed already handed out is skipped

@@ -39,76 +39,6 @@ struct Args {
     std::string inpSamF;
 };
 
-// EM.cpp:504-536 + BamWriter::work (BamWriter.h:82-146): every mapped alignment line (pair of lines for paired-end
-// reads) takes the next hit's posterior, in .dat order; all lines are written back, mates with read 1 first.
-void write_posterior_bam(const Args& a, const std::vector<TranscriptInfo>& tr, int ti_type, const HitStore& hits,
-                         std::vector<double>& post, const std::vector<double>& post0, int threads) {
-    if (a.bamSampling) {  // one alignment (or the noise entry) per read, drawn from its posterior (EM.cpp:507-531)
-        Mt engine(a.hasSeed ? a.seed : (uint32_t)time(NULL));
-        if (g_verbose) printf("Begin to sample reads from their posteriors.\n");
-        std::vector<double> arr;
-        for (uint64_t j = 0; j < hits.N; ++j) {
-            const uint64_t fr = hits.row_ptr[j], to = hits.row_ptr[j + 1];
-            const int len = (int)(to - fr + 1);
-            arr.assign(len, 0.0);
-            arr[0] = post0[j];
-            for (uint64_t k = fr; k < to; ++k) arr[k - fr + 1] = arr[k - fr] + post[k];
-            int id = -1;
-            if (!(arr[len - 1] < kEps)) {  // sample(): first index with arr[index] > u * total (sampling.h:50-65)
-                const double prb = engine.uniform01() * arr[len - 1];
-                int l = 0, r = len - 1;
-                while (l <= r) {
-                    const int mid = (l + r) / 2;
-                    if (arr[mid] <= prb) l = mid + 1;
-                    else r = mid - 1;
-                }
-                if (l >= len) die("sampling: the draw fell outside the cumulative posterior (reference: assert(l < len))");
-                id = l;
-            }
-            for (uint64_t k = fr; k < to; ++k) post[k] = ((int)(k - fr + 1) == id ? 1.0 : 0.0);
-        }
-        if (g_verbose) printf("Sampling is finished.\n");
-    }
-    AlnReader in(a.inpSamF);
-    const std::vector<int> e2i = map_bam_targets(in.ref_names(), tr, ti_type);
-    BamWriter out(a.outName + ".transcript.bam", rsem_bam_header_text(in.header_text()), threads);
-    const bool paired = a.read_type >= 2;
-    uint64_t next_hit = 0, cnt = 0;
-    auto take_hit = [&](const BamRecord& b) {
-        if (next_hit >= hits.H) die("The alignment file has more aligned lines than the .dat file has alignments (reference: assert(hit != NULL))!");
-        const int32_t t = b.tid();
-        if (t < 0 || t >= (int32_t)e2i.size() || e2i[t] != std::abs(hits.sid[next_hit]))
-            die("The alignment file does not match the .dat file (reference: assert(getInternalSid(tid + 1) == hit->getSid()))!");
-        return post[next_hit++];
-    };
-    BamRecord b, b2;
-    if (!paired) {
-        while (in.next(b)) {
-            ++cnt;
-            if (g_verbose && cnt % 1000000 == 0) printf("%llu alignment lines are loaded!\n", (unsigned long long)cnt);
-            if (b.mapped()) b.set_alignment_weight(take_hit(b));
-            out.write(b);
-        }
-    } else {
-        while (in.next(b) && in.next(b2)) {
-            cnt += 2;
-            if (g_verbose && cnt % 1000000 == 0) printf("%llu alignment lines are loaded!\n", (unsigned long long)cnt);
-            if (!b.read1()) b.data.swap(b2.data);
-            if (b.mapped() && b2.mapped()) {
-                const double w = take_hit(b);
-                if (b2.tid() != b.tid()) die("The two mates of a read pair align to different transcripts in the alignment file!");
-                b.set_alignment_weight(w);
-                b2.set_alignment_weight(w);
-            }
-            out.write(b);
-            out.write(b2);
-        }
-    }
-    if (next_hit != hits.H) die("The alignment file has fewer aligned lines than the .dat file has alignments (reference: assert(wrapper.getNextHit() == NULL))!");
-    out.close();
-    if (g_verbose) printf("Bam output file is generated!\n");
-}
-
 void usage() {
     printf("Usage : rsem-run-em refName read_type sampleName imdName statName [-p #Threads] [-b samInpF has_fai? [fai_file]] [-q] [--gibbs-out] [--sampling] [--seed seed] [--append-names]\n\n");
     printf("  refName: reference name\n");
@@ -398,23 +328,11 @@ int main(int argc, char* argv[]) {
     stamp(".ofg written");
     counts[0] += N0;
 
-    // ---- .theta (EM.cpp:484-500) ----
-    FILE* fo = fopen((a.statName + ".theta").c_str(), "w");
-    if (!fo) die("Cannot open " + a.statName + ".theta for writing!");
-    fprintf(fo, "%d\n", M + 1);
-    for (int i = 0; i < M; ++i) fprintf(fo, "%.15g ", theta[i]);
-    fprintf(fo, "%.15g\n", theta[M]);
-    calc_eel(refs, model.gld, eel);
-    polish_theta(theta, eel, model.mw);
-    for (int i = 0; i < M; ++i) fprintf(fo, "%.15g ", theta[i]);
-    fprintf(fo, "%.15g\n", theta[M]);
-    fclose(fo);
-
-    model.write(a.statName + ".model");
-    write_results_em(a.refName, a.imdName, transcripts, theta, eel, counts.data(), a.appendNames);
+    write_em_outputs(a.refName, a.imdName, a.statName, refs, transcripts, model, theta, counts, a.appendNames);
     stamp(".theta / .model / result rows written");
     if (a.genBam) {
-        write_posterior_bam(a, transcripts, ti_type, hits, post, post0, nThreads);
+        write_posterior_bam(a.inpSamF, a.outName, a.read_type, a.bamSampling, a.hasSeed, a.seed, transcripts, ti_type, hits,
+                            post, post0, nThreads, g_verbose);
         stamp("transcript BAM written");
     }
 

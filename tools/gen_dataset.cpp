@@ -74,6 +74,9 @@ struct Cfg {
                               // rsem-parse-alignments accepts (SamParser.h:122-265), for runs through rsem-calculate-expression
     int genome = 0;           // place every family on a chromosome as a gene locus: r.ti of type 0 with exon structures,
                               // and r.chrlist (rsem-tbam2gbam input).  Drawn from its own generator: the rest is unchanged
+    int has_sample_seed = 0;  // --sample-seed: the generator is reseeded after the reference and .omit are written, so
+    uint64_t sample_seed = 0; // samples share byte-identical ref/r.* and differ in expression and reads
+    double expressed_frac = 1.0;  // fraction of families with non-zero expression (single-cell-like samples)
 };
 
 const char BASES[5] = {'A', 'C', 'G', 'T', 'N'};
@@ -156,6 +159,8 @@ int main(int argc, char** argv) {
         else if (k == "--nfrac") c.nfrac = atof(v);
         else if (k == "--sam") c.sam = atoi(v);
         else if (k == "--genome") c.genome = atoi(v);
+        else if (k == "--sample-seed") { c.has_sample_seed = 1; c.sample_seed = strtoull(v, nullptr, 10); }
+        else if (k == "--expressed-frac") c.expressed_frac = atof(v);
         else { fprintf(stderr, "gen_dataset: unknown option %s\n", k.c_str()); return 2; }
     }
     const bool paired = c.read_type >= 2, hasQ = (c.read_type & 1);
@@ -298,12 +303,14 @@ int main(int argc, char** argv) {
     }
 
     // ---- expression weights --------------------------------------------------------------
+    if (c.has_sample_seed) g = Rng(c.sample_seed);
     std::vector<double> fam_cdf(F);
     int Fhit = 0;
     {
         double a = 0;
         for (int f = 0; f < F; ++f) {
             bool hittable = fam_start[f] <= Mhit;
+            if (c.expressed_frac < 1.0 && f > 0 && g.uni() >= c.expressed_frac) hittable = false;   // family 0 stays expressed
             double u = g.uni();
             a += hittable ? u * u * u * u + 1e-6 : 0.0;
             fam_cdf[f] = a;
