@@ -255,6 +255,54 @@ int rsem_b200_gibbs_split_chains(int32_t n_chains, const int32_t* chain_samples,
  * completed upload, or src == dst, is refused with RSEM_B200_ERR_ARG.                                                */
 int rsem_b200_gibbs_upload_from(rsem_b200_ctx* dst, const rsem_b200_ctx* src);
 
+/* ---- K13: the Gibbs chains of many samples at once (rsem-run-gibbs-batch) --------------------------------------------
+ * A Gibbs batch holds the .ofg matrices of several samples, their per-sample inputs (rsem_b200_gibbs_params) and room for
+ * their outputs in one device arena, and runs every (sample, chain) job in one cooperative launch.  A team of
+ * worker_ctas worker CTAs and 1 generator CTA runs one job at a time with the component-parallel chain of
+ * rsem_b200_gibbs_run_chains; teams claim jobs from a device counter, largest first (sweeps x reads).  A job's count
+ * vectors and chain_acc block are bit-identical to that chain run by rsem_b200_gibbs_run_chains on the sample alone.
+ *
+ * Size rule: a sample takes the batch when 1248 <= N1 <= 2^19 reads.  Smaller ones run the serial kernel of
+ * rsem_b200_gibbs_run_chains (its generator runs one sweep ahead, which needs 624 outputs to span at most two sweeps);
+ * larger ones have enough reads to spread over a whole-GPU cooperative launch of their own, which one team cannot use.
+ * Both are refused with RSEM_B200_ERR_UNSUPPORTED and run with rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains.
+ * The batch lives on `ctx`'s device and stream; destroy it before the context.                                        */
+typedef struct rsem_b200_gibbs_batch rsem_b200_gibbs_batch;
+#define RSEM_B200_GIBBS_BATCH_MIN_READS 1248ull
+#define RSEM_B200_GIBBS_BATCH_MAX_READS 524288ull
+/* capacity_bytes = 0: half of the device memory free at the call.  worker_ctas: worker CTAs per team, 1..8, or 0 for the
+ * library's choice (2).                                                                                                */
+int rsem_b200_gibbs_batch_create(rsem_b200_ctx* ctx, uint64_t capacity_bytes, int32_t worker_ctas,
+                                 rsem_b200_gibbs_batch** out);
+int rsem_b200_gibbs_batch_destroy(rsem_b200_gibbs_batch* batch);
+/* Arena bytes of a sample of N1 reads, E entries, M transcripts, n_genes genes and n_samples count vectors over n_chains
+ * chains (layout, inputs, count vectors, per-chain sums and state), or RSEM_B200_ERR_UNSUPPORTED outside the size rule
+ * above.  No GPU needed.                                                                                               */
+int rsem_b200_gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes, int32_t n_samples,
+                                       int32_t n_chains, uint64_t* bytes);
+/* Adds a sample: its .ofg matrix as for rsem_b200_gibbs_upload and its chains' parameters (copied; every pointer of
+ * params is read during the call only).  Every sample of a batch has the M and n_genes of the first.  Refused with
+ * RSEM_B200_ERR_ARG for a read without entries or a bad id, RSEM_B200_ERR_FULL when the arena has no room left,
+ * RSEM_B200_ERR_UNSUPPORTED outside the size rule.  *slot receives its handle.                                          */
+int rsem_b200_gibbs_batch_add(rsem_b200_gibbs_batch* batch, uint64_t N1, uint64_t E, const uint64_t* row_ptr,
+                              const int32_t* sid, const double* conprb, const rsem_b200_gibbs_params* params,
+                              int32_t* slot);
+typedef struct rsem_b200_gibbs_batch_stats {
+    double device_ms;         /* CUDA events around the launch                                                        */
+    int32_t worker_ctas;      /* worker CTAs per team                                                                 */
+    int32_t teams;            /* co-resident teams of the launch                                                      */
+    int64_t jobs;             /* (sample, chain) jobs run                                                             */
+    uint64_t chain_cycles;    /* SM cycles of worker CTA 0 summed over the jobs: whole sweeps (ChainSync::prof[0,2,3]) */
+    uint64_t sample_cycles;   /* of which the per-kept-draw O(M) work (ChainSync::prof[3])                            */
+} rsem_b200_gibbs_batch_stats;
+/* Runs every sample added since the last run, in one launch.  stats may be NULL. */
+int rsem_b200_gibbs_batch_run(rsem_b200_gibbs_batch* batch, rsem_b200_gibbs_batch_stats* stats);
+/* A sample's outputs after its run, as rsem_b200_gibbs_run_chains gives them: count_vectors (sum of chain_samples
+ * vectors of M + 1), chain_acc (n_chains blocks of 4 (M + 1) + n_genes).                                              */
+int rsem_b200_gibbs_batch_result(rsem_b200_gibbs_batch* batch, int32_t slot, int32_t* count_vectors, double* chain_acc);
+/* Frees every sample (the arena is empty again). */
+int rsem_b200_gibbs_batch_clear(rsem_b200_gibbs_batch* batch);
+
 typedef struct rsem_b200_sim_stats rsem_b200_sim_stats;
 
 /* ---- read simulation (rsem-simulate-reads, simulation.cpp:86-130) ------------------------------

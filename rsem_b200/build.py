@@ -3,7 +3,7 @@
   rsem_b200/librsem_b200.so   CUDA kernels + C ABI, sm_90a only
   bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments, bin/rsem-simulate-reads,
   bin/rsem-calculate-credibility-intervals, bin/rsem-for-ebseq-calculate-clustering-info, bin/rsem-tbam2gbam,
-  bin/rsem-bam2wig, bin/rsem-bam2readdepth, bin/rsem-run-em-batch
+  bin/rsem-bam2wig, bin/rsem-bam2readdepth, bin/rsem-run-em-batch, bin/rsem-run-gibbs-batch
                               C++ drop-in executables (link the .so)
   tools/gen_dataset           synthetic intermediate-file generator (tooling)
   oracle/librsem_oracle.so    CPU restatement (test infrastructure)
@@ -70,7 +70,8 @@ def build_host(force: bool = False):
                 "main_ci.cpp": "rsem-calculate-credibility-intervals",
                 "main_clustering_info.cpp": "rsem-for-ebseq-calculate-clustering-info",
                 "main_tbam2gbam.cpp": "rsem-tbam2gbam", "main_bam2wig.cpp": "rsem-bam2wig",
-                "main_bam2readdepth.cpp": "rsem-bam2readdepth", "main_em_batch.cpp": "rsem-run-em-batch"}[os.path.basename(m)]
+                "main_bam2readdepth.cpp": "rsem-bam2readdepth", "main_em_batch.cpp": "rsem-run-em-batch",
+                "main_gibbs_batch.cpp": "rsem-run-gibbs-batch"}[os.path.basename(m)]
         out = os.path.join(ROOT, "bin", name)
         ffm_use = {"rsem-simulate-reads": "sim_tables.o", "rsem-calculate-credibility-intervals": "ci_sample.o"}
         extra = [o for o in ffm_objs if os.path.basename(o) == ffm_use.get(name)]

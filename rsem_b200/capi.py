@@ -57,6 +57,11 @@ class GibbsStats(C.Structure):
     _fields_ = [("device_ms", C.c_double), ("worker_ctas", C.c_int32), ("launches", C.c_int32)]
 
 
+class GibbsBatchStats(C.Structure):
+    _fields_ = [("device_ms", C.c_double), ("worker_ctas", C.c_int32), ("teams", C.c_int32), ("jobs", C.c_int64),
+                ("chain_cycles", C.c_uint64), ("sample_cycles", C.c_uint64)]
+
+
 class SimParams(C.Structure):
     _fields_ = [("model_type", C.c_int32), ("M", C.c_int32), ("seed", C.c_uint32), ("exact_body", C.c_int32),
                 ("N", C.c_uint64), ("window_words", C.c_uint64), ("theta_cdf", C.POINTER(C.c_double)),
@@ -137,10 +142,16 @@ SYMBOLS = [
     "rsem_b200_gbam_convert", "rsem_b200_wig_depth", "rsem_b200_gibbs_run_chains", "rsem_b200_gibbs_sum_chains",
     "rsem_b200_gibbs_split_chains", "rsem_b200_gibbs_upload_from", "rsem_b200_batch_create", "rsem_b200_batch_destroy",
     "rsem_b200_batch_sample_bytes", "rsem_b200_batch_add", "rsem_b200_batch_run", "rsem_b200_batch_slots",
-    "rsem_b200_batch_final", "rsem_b200_batch_remove", "rsem_b200_batch_timing",
+    "rsem_b200_batch_final", "rsem_b200_batch_remove", "rsem_b200_batch_timing", "rsem_b200_gibbs_batch_create",
+    "rsem_b200_gibbs_batch_destroy", "rsem_b200_gibbs_batch_sample_bytes", "rsem_b200_gibbs_batch_add",
+    "rsem_b200_gibbs_batch_run", "rsem_b200_gibbs_batch_result", "rsem_b200_gibbs_batch_clear",
 ]
 
+RSEM_B200_ERR_ARG = 2
+RSEM_B200_ERR_UNSUPPORTED = 4
 RSEM_B200_ERR_FULL = 5
+GIBBS_BATCH_MIN_READS = 1248
+GIBBS_BATCH_MAX_READS = 524288
 
 
 class Lib:
@@ -549,3 +560,65 @@ class Batch:
         ms, n = C.c_double(0), C.c_uint64(0)
         self.lib.check(self.lib.dll.rsem_b200_batch_timing(self._h, C.byref(ms), C.byref(n)))
         return ms.value, n.value
+
+
+class GibbsBatch:
+    """K13: the Gibbs chains of many samples in one cooperative launch (include/rsem_b200.h, rsem_b200_gibbs_batch_*)."""
+
+    def __init__(self, ctx: Context, capacity_bytes: int = 0, worker_ctas: int = 0):
+        self.lib = ctx.lib
+        self.ctx = ctx   # the batch lives on the context's device and stream
+        self._h = C.c_void_p()
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_batch_create(ctx._h, C.c_uint64(capacity_bytes), C.c_int32(worker_ctas),
+                                                                 C.byref(self._h)))
+        self.shapes = {}
+
+    def close(self):
+        if self._h:
+            self.lib.dll.rsem_b200_gibbs_batch_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def sample_bytes(self, N1: int, E: int, M: int, n_genes: int, n_samples: int, n_chains: int) -> int:
+        out = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_batch_sample_bytes(
+            C.c_uint64(N1), C.c_uint64(E), C.c_int32(M), C.c_int32(n_genes), C.c_int32(n_samples), C.c_int32(n_chains),
+            C.byref(out)))
+        return out.value
+
+    def add(self, row_ptr, sid, conprb, params: GibbsParams) -> int:
+        """returns the slot; raises RsemB200Error with .code (RSEM_B200_ERR_FULL, RSEM_B200_ERR_UNSUPPORTED, ...)"""
+        row_ptr, sid, conprb = _arr(row_ptr, np.uint64), _arr(sid, np.int32), _arr(conprb, np.float64)
+        slot = C.c_int32(-1)
+        rc = self.lib.dll.rsem_b200_gibbs_batch_add(self._h, C.c_uint64(len(row_ptr) - 1), C.c_uint64(len(sid)),
+                                                    _p(row_ptr, C.c_uint64), _p(sid, C.c_int32), _dp(conprb),
+                                                    C.byref(params), C.byref(slot))
+        if rc != 0:
+            err = RsemB200Error(f"librsem_b200 error {rc}: {self.lib.dll.rsem_b200_last_error().decode()}")
+            err.code = rc
+            raise err
+        samples = [params.chain_samples[t] for t in range(params.n_chains)]
+        self.shapes[slot.value] = (params.M, params.n_genes, samples)
+        return slot.value
+
+    def run(self) -> GibbsBatchStats:
+        stats = GibbsBatchStats()
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_batch_run(self._h, C.byref(stats)))
+        return stats
+
+    def result(self, slot: int):
+        """(count vectors: int32 sum(chain_samples) x (M + 1), chain_acc: float64 n_chains x (4 (M + 1) + n_genes))"""
+        M, n_genes, samples = self.shapes[slot]
+        cv = np.zeros((sum(samples), M + 1), np.int32)
+        acc = np.zeros((len(samples), 4 * (M + 1) + n_genes))
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_batch_result(self._h, C.c_int32(slot), _p(cv, C.c_int32), _dp(acc)))
+        return cv, acc
+
+    def clear(self):
+        self.lib.check(self.lib.dll.rsem_b200_gibbs_batch_clear(self._h))
+        self.shapes = {}

@@ -831,6 +831,49 @@ int rsem_b200_gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, rsem_
     return rsem_b200_gibbs_sum_chains(p, acc.data(), out);
 }
 
+int rsem_b200_gibbs_batch_create(rsem_b200_ctx* c, uint64_t capacity_bytes, int32_t worker_ctas, rsem_b200_gibbs_batch** out) {
+    RB_ARG(c && out, "NULL argument");
+    return gibbs_batch_create(c, capacity_bytes, worker_ctas, out);
+}
+
+int rsem_b200_gibbs_batch_destroy(rsem_b200_gibbs_batch* b) {
+    if (b) gibbs_batch_destroy(b);
+    return 0;
+}
+
+int rsem_b200_gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes, int32_t n_samples,
+                                       int32_t n_chains, uint64_t* bytes) {
+    RB_ARG(bytes, "NULL argument");
+    RB_ARG(M >= 0 && n_genes >= 0 && n_samples >= 1 && n_chains >= 1, "bad sizes");
+    return gibbs_batch_sample_bytes(N1, E, M, n_genes, n_samples, n_chains, bytes);
+}
+
+int rsem_b200_gibbs_batch_add(rsem_b200_gibbs_batch* b, uint64_t N1, uint64_t E, const uint64_t* row_ptr, const int32_t* sid,
+                              const double* conprb, const rsem_b200_gibbs_params* p, int32_t* slot) {
+    RB_ARG(b && p && slot && row_ptr && (E == 0 || (sid && conprb)), "NULL argument");
+    RB_ARG(row_ptr[0] == 0 && row_ptr[N1] == E, "row_ptr must start at 0 and end at E");
+    RB_ARG(p->M >= 0 && p->n_genes >= 0 && p->burnin >= 0 && p->gap >= 1, "bad parameters");
+    RB_ARG(p->n_chains >= 1 && p->chain_samples && p->chain_seeds && p->init_counts && p->pseudo_counts && p->eel && p->mw &&
+               p->gene_start, "bad chain parameters");
+    return gibbs_batch_add(b, N1, E, row_ptr, sid, conprb, p, slot);
+}
+
+int rsem_b200_gibbs_batch_run(rsem_b200_gibbs_batch* b, rsem_b200_gibbs_batch_stats* stats) {
+    RB_ARG(b, "NULL argument");
+    return gibbs_batch_run(b, stats);
+}
+
+int rsem_b200_gibbs_batch_result(rsem_b200_gibbs_batch* b, int32_t slot, int32_t* count_vectors, double* chain_acc) {
+    RB_ARG(b && count_vectors && chain_acc, "NULL argument");
+    return gibbs_batch_result(b, slot, count_vectors, chain_acc);
+}
+
+int rsem_b200_gibbs_batch_clear(rsem_b200_gibbs_batch* b) {
+    RB_ARG(b, "NULL argument");
+    gibbs_batch_clear(b);
+    return 0;
+}
+
 int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
     RB_ARG(c && p, "NULL argument");
     RB_ARG(p->model_type >= 0 && p->model_type <= 3 && p->M >= 1, "bad model type or M");

@@ -349,6 +349,31 @@ int model_launch_update(rsem_b200_ctx* ctx);
 int gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
               rsem_b200_gibbs_stats* stats);
 int gibbs_prepare(rsem_b200_ctx* ctx, const uint64_t* row_ptr, const int32_t* sid);
+// host side of the component-parallel sampler's layout (gibbs_kernels.cu): components, segments longest first, local
+// ids of register-resident components, rows in slot order.  gibbs_prepare and the Gibbs batch (K13) both build it.
+struct GibbsLayout {
+    uint64_t N1 = 0;
+    std::vector<int32_t> order;        // N1 read ids in slot order
+    std::vector<uint64_t> p_off;       // N1 + 1 entry offsets of the slots
+    std::vector<int32_t> p_sid;        // E ids (local ids in register-resident components)
+    std::vector<int32_t> seg_start;    // n_segs + 1
+    std::vector<int32_t> seg_ntr;      // n_segs
+    std::vector<int32_t> seg_tid_off;  // n_segs + 1
+    std::vector<int32_t> comp_tids;
+    int32_t n_segs = 0;
+    uint32_t max_len = 0;
+    bool empty_row = false;
+};
+int gibbs_layout(const uint64_t* row_ptr, const int32_t* sid, uint64_t N1, int M, GibbsLayout& L);
+int gibbs_batch_create(rsem_b200_ctx* c, uint64_t capacity, int worker_ctas, rsem_b200_gibbs_batch** out);
+void gibbs_batch_destroy(rsem_b200_gibbs_batch* b);
+int gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes, int32_t n_samples, int32_t n_chains,
+                             uint64_t* bytes);
+int gibbs_batch_add(rsem_b200_gibbs_batch* b, uint64_t N1, uint64_t E, const uint64_t* row_ptr, const int32_t* sid,
+                    const double* conprb, const rsem_b200_gibbs_params* p, int32_t* slot);
+int gibbs_batch_run(rsem_b200_gibbs_batch* b, rsem_b200_gibbs_batch_stats* stats);
+int gibbs_batch_result(rsem_b200_gibbs_batch* b, int32_t slot, int32_t* count_vectors, double* chain_acc);
+void gibbs_batch_clear(rsem_b200_gibbs_batch* b);
 
 // sim_kernels.cu
 int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p);

@@ -910,16 +910,17 @@ __device__ __forceinline__ void walk_pass_converged(const PArgs& a, ChainSync* s
     }
 }
 
+// One chain on the CTAs of its team: worker CTAs 0 .. ctas_per_chain - 1 and the generator CTA (cta == ctas_per_chain).
+// `chain` indexes what belongs to the chain (chain_samples, chain_seeds, chain_cv_offset, sync, slice_tot, acc), `slot` the
+// scratch it runs in (counts, counts_start, z, ubuf, flips, pre, theta_tmp).  gibbs_parallel_kernel runs chain c in slot c;
+// gibbs_batch_kernel runs a job's chain of its sample in slot 0 of a PArgs whose scratch pointers are the team's.
 template <int PF>   // 0: row-at-a-time walk, 1: pipelined walk per segment, 2: pipelined, both groups of a warp in one loop
-__global__ void __launch_bounds__(kPThreads, PF ? 3 : 4) gibbs_parallel_kernel(const PArgs a) {
+__device__ __forceinline__ void chain_body(const PArgs& a, const int chain, const size_t slot, const unsigned cta) {
     __shared__ EntryRing sh_ring[PF ? kPThreads / kGL : 1];
     __shared__ double sh_red[kPThreads / 32];
     __shared__ int sh_scan[kPThreads];
     __shared__ int sh_base[512];     // exclusive prefix of the slice totals (<= 512 worker CTAs per chain)
     __shared__ GroupSmem sh_grp[kPThreads / kGL];
-    const unsigned group = a.ctas_per_chain + 1;   // worker CTAs + the generator CTA
-    const int chain = a.chain_base + blockIdx.x / group;
-    const unsigned cta = blockIdx.x % group;
     const unsigned n_ctas = a.ctas_per_chain;
     const int tid = threadIdx.x;
     const int M1 = a.M + 1;
@@ -928,20 +929,20 @@ __global__ void __launch_bounds__(kPThreads, PF ? 3 : 4) gibbs_parallel_kernel(c
     const int n_samples = a.chain_samples[chain];
     const int chainlen = 1 + (n_samples - 1) * a.gap;
     const unsigned n_sweeps = 1u + (unsigned)(a.burnin + chainlen);   // sweep 0 = initial state from conprb alone
-    unsigned* ubuf = a.ubuf + (size_t)chain * 2 * a.N1;
+    unsigned* ubuf = a.ubuf + slot * 2 * a.N1;
     if (cta == n_ctas) {
         generator_loop(a, sy, ubuf, n_sweeps, a.chain_seeds[chain]);
         return;
     }
     const unsigned chain_threads = n_ctas * kPThreads, ctid = cta * kPThreads + tid;
-    int* counts = a.counts + (size_t)chain * M1;
-    int* counts_start = a.counts_start + (size_t)chain * M1;
-    int* zbuf = a.z + (size_t)chain * 2 * a.N1;
-    unsigned* fl = a.flips + (size_t)chain * 4 * W;
-    int* pre = a.pre + (size_t)chain * W;
+    int* counts = a.counts + slot * M1;
+    int* counts_start = a.counts_start + slot * M1;
+    int* zbuf = a.z + slot * 2 * a.N1;
+    unsigned* fl = a.flips + slot * 4 * W;
+    int* pre = a.pre + slot * W;
     int* slice_tot = a.slice_tot + (size_t)chain * n_ctas;
     double* acc = a.acc + (size_t)chain * (4 * (size_t)M1 + a.n_genes);
-    double* theta = a.theta_tmp + (size_t)chain * 2 * M1;
+    double* theta = a.theta_tmp + slot * 2 * M1;
     double* fpkm = theta + M1;
     int* cv = a.count_vectors + a.chain_cv_offset[chain] * M1;
     // this CTA's slice of flip words (prefix sums are formed per slice, the slice bases are added on the fly)
@@ -1128,6 +1129,78 @@ __global__ void __launch_bounds__(kPThreads, PF ? 3 : 4) gibbs_parallel_kernel(c
     }
 }
 
+template <int PF>
+__global__ void __launch_bounds__(kPThreads, PF ? 3 : 4) gibbs_parallel_kernel(const PArgs a) {
+    const unsigned group = a.ctas_per_chain + 1;   // worker CTAs + the generator CTA
+    const int chain = a.chain_base + blockIdx.x / group;
+    chain_body<PF>(a, chain, (size_t)chain, blockIdx.x % group);
+}
+
+// ---- K13: the chains of many samples in one cooperative launch (rsem_b200_gibbs_batch_*) -----------------------------
+// A job is one (sample, chain); a team is k worker CTAs + 1 generator CTA, the shape of one chain of gibbs_parallel_kernel.
+// Worker CTA 0 of a team claims the next job from a device counter (jobs are numbered largest first) and hands its number
+// to the team's other CTAs through the team's mailbox word (claim number << 32 | job).  Every CTA then copies the job's
+// sample view into shared memory - the sample's PArgs with the team's scratch in slot 0 - and runs chain_body<2> on it.
+// A job's ChainSync and slice totals belong to the job (zeroed before the launch): a team starts every job fresh.  The
+// team's CTAs have all read claim r before worker CTA 0 can post claim r + 1: the workers passed the job's first barrier
+// and the generator published the job's first uniforms, both of which worker CTA 0 waits for.
+struct BArgs {
+    const PArgs* samples;
+    const int2* jobs;                 // (sample, chain of the sample), largest first
+    unsigned n_jobs, k;
+    unsigned* next_job;
+    unsigned long long* mailbox;      // one word per team
+    // per team scratch, sized for the largest sample of the launch
+    int* counts;
+    int* counts_start;
+    int* z;
+    unsigned* ubuf;
+    unsigned* flips;
+    int* pre;
+    double* theta_tmp;
+    unsigned long long n1_max;
+    unsigned w_max;
+    int M1;
+};
+
+__global__ void __launch_bounds__(kPThreads, 3) gibbs_batch_kernel(const BArgs b) {
+    __shared__ PArgs sa;
+    __shared__ unsigned sh_job;
+    const unsigned group = b.k + 1;
+    const unsigned team = blockIdx.x / group, cta = blockIdx.x % group;
+    unsigned long long* box = b.mailbox + team;
+    for (unsigned long long r = 1;; ++r) {
+        if (threadIdx.x == 0) {
+            unsigned job;
+            if (cta == 0) {
+                job = atomicAdd(b.next_job, 1u);
+                atomicExch(box, (r << 32) | job);
+            } else {
+                unsigned long long v;
+                while (((v = *((volatile unsigned long long*)box)) >> 32) != r) {}
+                job = (unsigned)v;
+            }
+            sh_job = job;
+            if (job < b.n_jobs) {
+                const int2 jb = b.jobs[job];
+                sa = b.samples[jb.x];
+                sa.counts = b.counts + (size_t)team * b.M1;
+                sa.counts_start = b.counts_start + (size_t)team * b.M1;
+                sa.z = b.z + (size_t)team * 2 * b.n1_max;
+                sa.ubuf = b.ubuf + (size_t)team * 2 * b.n1_max;
+                sa.flips = b.flips + (size_t)team * 4 * b.w_max;
+                sa.pre = b.pre + (size_t)team * b.w_max;
+                sa.theta_tmp = b.theta_tmp + (size_t)team * 2 * b.M1;
+                sa.chain_base = jb.y;
+            }
+        }
+        __syncthreads();
+        if (sh_job >= b.n_jobs) return;
+        chain_body<2>(sa, sa.chain_base, 0, cta);
+        __syncthreads();   // sa and sh_job are rewritten by the next claim
+    }
+}
+
 template <class T>
 int to_dev(T** d, const T* h, size_t n, cudaStream_t s) {
     RB_CUDA(cudaMalloc(d, std::max<size_t>(n, 1) * sizeof(T)));
@@ -1234,10 +1307,9 @@ __global__ void permute_rows_kernel(const unsigned long long* row_ptr, const dou
 }
 
 // ---- static preparation for the component-parallel sampler (host) ---------------------------------------------
-int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid) {
-    DevGibbs& g = c->gibbs;
-    const uint64_t N1 = g.N1;
-    const int M = g.M;
+int gibbs_layout(const uint64_t* row_ptr, const int32_t* sid, uint64_t N1, int M, GibbsLayout& L) {
+    L = GibbsLayout{};
+    L.N1 = N1;
     if (N1 == 0) return 0;
     if (N1 > 0x7fffffffull) { set_error("gibbs: more than 2^31 reads are not supported"); return RSEM_B200_ERR_UNSUPPORTED; }
     // connected components of the read x transcript graph, noise transcript excluded (union-find with path halving)
@@ -1251,7 +1323,7 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
     for (uint64_t i = 0; i < N1; ++i) {
         int32_t first = 0;
         max_len = std::max(max_len, row_ptr[i + 1] - row_ptr[i]);
-        if (row_ptr[i + 1] == row_ptr[i]) g.empty_row = true;
+        if (row_ptr[i + 1] == row_ptr[i]) L.empty_row = true;
         for (uint64_t j = row_ptr[i]; j < row_ptr[i + 1]; ++j) {
             const int32_t t = sid[j];
             if (t < 0 || t > M) { set_error("gibbs: transcript id out of range in the .ofg matrix"); return RSEM_B200_ERR_ARG; }
@@ -1263,7 +1335,7 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
             }
         }
     }
-    g.max_len = (uint32_t)max_len;
+    L.max_len = (uint32_t)max_len;
     // component of a read = root of its first non-noise transcript; 0 = the row holds only the noise entry (its own segment)
     std::vector<int32_t> comp(N1);
     std::vector<uint32_t> comp_reads((size_t)M + 1, 0);
@@ -1280,76 +1352,91 @@ int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid)
     std::vector<int32_t> roots;
     for (int t = 1; t <= M; ++t) if (comp_reads[t]) roots.push_back(t);
     std::stable_sort(roots.begin(), roots.end(), [&](int32_t x, int32_t y) { return comp_reads[x] > comp_reads[y]; });
-    std::vector<int32_t> seg_start;
+    std::vector<int32_t>& seg_start = L.seg_start;
     seg_start.reserve(roots.size() + n_lonely + 1);
     std::vector<uint64_t> fill((size_t)M + 1, 0);
     uint64_t at = 0;
     for (int32_t r : roots) { seg_start.push_back((int32_t)at); fill[r] = at; at += comp_reads[r]; }
-    std::vector<int32_t> order(N1);
+    std::vector<int32_t>& order = L.order;
+    order.resize(N1);
     for (uint64_t i = 0; i < N1; ++i) {
         if (comp[i]) order[fill[comp[i]]++] = (int32_t)i;
         else { seg_start.push_back((int32_t)at); order[at++] = (int32_t)i; }
     }
     seg_start.push_back((int32_t)N1);
-    g.n_segs = (int32_t)seg_start.size() - 1;
+    L.n_segs = (int32_t)seg_start.size() - 1;
     // transcripts of every component (sorted) and the local id of a transcript inside its component (1.., 0 = noise):
     // components of fewer than 32 transcripts are walked with their counts in registers, rows and assignments in local ids
     std::vector<int32_t> lid((size_t)M + 1, 0), ntr((size_t)M + 1, 0);
     for (int t = 1; t <= M; ++t) lid[t] = ++ntr[find(t)];
-    std::vector<int32_t> seg_ntr(g.n_segs, 0), seg_tid_off(g.n_segs + 1, 0), comp_tids;
+    L.seg_ntr.assign(L.n_segs, 0);
+    L.seg_tid_off.assign(L.n_segs + 1, 0);
     {
         std::vector<int32_t> tid_at((size_t)M + 1, 0);   // offset of root r's list
         int32_t at_t = 0;
         for (size_t sgi = 0; sgi < roots.size(); ++sgi) {
-            seg_ntr[sgi] = ntr[roots[sgi]];
-            seg_tid_off[sgi] = at_t;
+            L.seg_ntr[sgi] = ntr[roots[sgi]];
+            L.seg_tid_off[sgi] = at_t;
             tid_at[roots[sgi]] = at_t;
             at_t += ntr[roots[sgi]];
         }
-        for (int sgi = (int)roots.size(); sgi <= g.n_segs; ++sgi) seg_tid_off[sgi] = at_t;
-        comp_tids.assign((size_t)at_t + 1, 0);
+        for (int sgi = (int)roots.size(); sgi <= L.n_segs; ++sgi) L.seg_tid_off[sgi] = at_t;
+        L.comp_tids.assign((size_t)at_t + 1, 0);
         for (int t = 1; t <= M; ++t) {
             const int32_t r = find(t);
-            if (comp_reads[r]) comp_tids[(size_t)tid_at[r] + lid[t] - 1] = t;
+            if (comp_reads[r]) L.comp_tids[(size_t)tid_at[r] + lid[t] - 1] = t;
         }
     }
     // rows re-laid in slot order so that a segment is one contiguous stream
+    const uint64_t E = row_ptr[N1];
+    L.p_off.resize(N1 + 1);
+    L.p_sid.resize(E);
+    L.p_off[0] = 0;
+    for (uint64_t q = 0; q < N1; ++q) L.p_off[q + 1] = L.p_off[q] + (row_ptr[order[q] + 1] - row_ptr[order[q]]);
+    for (uint64_t q = 0; q < N1; ++q) {
+        const uint64_t src = row_ptr[order[q]], n = row_ptr[order[q] + 1] - src;
+        const int32_t k = comp[order[q]];
+        if (k == 0 || ntr[k] < 32) {   // register-resident component: local ids
+            for (uint64_t j = 0; j < n; ++j) L.p_sid[L.p_off[q] + j] = lid[sid[src + j]];
+        } else memcpy(L.p_sid.data() + L.p_off[q], sid + src, n * sizeof(int32_t));
+    }
+    return 0;
+}
+
+int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid) {
+    DevGibbs& g = c->gibbs;
+    const uint64_t N1 = g.N1;
+    if (N1 == 0) return 0;
+    GibbsLayout L;
+    if (int rc = gibbs_layout(row_ptr, sid, N1, g.M, L)) return rc;
+    g.max_len = L.max_len;
+    g.empty_row = L.empty_row;
+    g.n_segs = L.n_segs;
     {
         const uint64_t E = row_ptr[N1];
-        std::vector<uint64_t> p_off(N1 + 1);
-        std::vector<int32_t> p_sid(E);
-        p_off[0] = 0;
-        for (uint64_t q = 0; q < N1; ++q) p_off[q + 1] = p_off[q] + (row_ptr[order[q] + 1] - row_ptr[order[q]]);
-        for (uint64_t q = 0; q < N1; ++q) {
-            const uint64_t src = row_ptr[order[q]], n = row_ptr[order[q] + 1] - src;
-            const int32_t k = comp[order[q]];
-            if (k == 0 || ntr[k] < 32) {   // register-resident component: local ids
-                for (uint64_t j = 0; j < n; ++j) p_sid[p_off[q] + j] = lid[sid[src + j]];
-            } else memcpy(p_sid.data() + p_off[q], sid + src, n * sizeof(int32_t));
-        }
         RB_CUDA(cudaMalloc(&g.p_off, (N1 + 1) * sizeof(uint64_t)));
         RB_CUDA(cudaMalloc(&g.p_sid, (E + 16) * sizeof(int32_t)));
         RB_CUDA(cudaMalloc(&g.p_con, (E + 16) * sizeof(double)));
-        RB_CUDA(cudaMemcpyAsync(g.p_off, p_off.data(), (N1 + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
-        RB_CUDA(cudaMemcpyAsync(g.p_sid, p_sid.data(), E * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        RB_CUDA(cudaMemcpyAsync(g.p_off, L.p_off.data(), (N1 + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
+        RB_CUDA(cudaMemcpyAsync(g.p_sid, L.p_sid.data(), E * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
         // conprb is permuted on the device from the already uploaded copy
         RB_CUDA(cudaMalloc(&g.order, N1 * sizeof(int32_t)));
-        RB_CUDA(cudaMemcpyAsync(g.order, order.data(), N1 * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        RB_CUDA(cudaMemcpyAsync(g.order, L.order.data(), N1 * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
         permute_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(reinterpret_cast<const unsigned long long*>(g.row_ptr), g.conprb,
                                                                    g.order, reinterpret_cast<const unsigned long long*>(g.p_off), N1, g.p_con);
         RB_CUDA(cudaGetLastError());
         c->launches++;
         RB_CUDA(cudaStreamSynchronize(c->stream));
     }
-    RB_CUDA(cudaMalloc(&g.seg_start, seg_start.size() * sizeof(int32_t)));
-    RB_CUDA(cudaMemcpyAsync(g.seg_start, seg_start.data(), seg_start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMalloc(&g.seg_ntr, std::max<size_t>(seg_ntr.size(), 1) * sizeof(int32_t)));
-    RB_CUDA(cudaMalloc(&g.seg_tid_off, seg_tid_off.size() * sizeof(int32_t)));
-    RB_CUDA(cudaMalloc(&g.comp_tids, comp_tids.size() * sizeof(int32_t)));
-    g.n_comp_tids = comp_tids.size();
-    RB_CUDA(cudaMemcpyAsync(g.seg_ntr, seg_ntr.data(), seg_ntr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(g.seg_tid_off, seg_tid_off.data(), seg_tid_off.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(g.comp_tids, comp_tids.data(), comp_tids.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMalloc(&g.seg_start, L.seg_start.size() * sizeof(int32_t)));
+    RB_CUDA(cudaMemcpyAsync(g.seg_start, L.seg_start.data(), L.seg_start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMalloc(&g.seg_ntr, std::max<size_t>(L.seg_ntr.size(), 1) * sizeof(int32_t)));
+    RB_CUDA(cudaMalloc(&g.seg_tid_off, L.seg_tid_off.size() * sizeof(int32_t)));
+    RB_CUDA(cudaMalloc(&g.comp_tids, L.comp_tids.size() * sizeof(int32_t)));
+    g.n_comp_tids = L.comp_tids.size();
+    RB_CUDA(cudaMemcpyAsync(g.seg_ntr, L.seg_ntr.data(), L.seg_ntr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMemcpyAsync(g.seg_tid_off, L.seg_tid_off.data(), L.seg_tid_off.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMemcpyAsync(g.comp_tids, L.comp_tids.data(), L.comp_tids.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
     RB_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -1487,6 +1574,346 @@ int gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_
     // tiny inputs: a 624-word regeneration would span more than two sweeps (the generator runs only one sweep ahead)
     if (c->gibbs.N1 < 1248 || !c->gibbs.order) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
     return gibbs_run_parallel(c, p, count_vectors, chain_acc, stats);
+}
+
+// ---- K13 host side ------------------------------------------------------------------------------------------------------
+namespace {
+constexpr int kBatchMaxWorkers = 8;   // worker CTAs per team; slice totals are sized for it
+constexpr int kBatchDefaultWorkers = 2;
+
+size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// byte offsets of a sample's parts in its block; n_segs <= N1 and comp_tids <= M + 1 bound the layout before it is built
+struct GParts {
+    size_t order, p_off, p_sid, p_con, seg_start, seg_ntr, seg_tid_off, comp_tids, init, alpha, eel, mw, gene, samples, seeds,
+        cv_off, head, sync, slice_tot, acc, zero_end, cv, total;
+};
+GParts gparts(uint64_t N1, uint64_t E, int M, int n_genes, int n_samples, int n_chains) {
+    const size_t M1 = (size_t)M + 1;
+    GParts p{};
+    size_t at = 0;
+    auto put = [&](size_t& off, size_t bytes) { off = at; at = align_up(at + bytes); };
+    put(p.order, N1 * 4);
+    put(p.p_off, (N1 + 1) * 8);
+    put(p.p_sid, (E + 16) * 4);
+    put(p.p_con, (E + 16) * 8);
+    put(p.seg_start, (N1 + 1) * 4);
+    put(p.seg_ntr, std::max<uint64_t>(N1, 1) * 4);
+    put(p.seg_tid_off, (N1 + 1) * 4);
+    put(p.comp_tids, (M1 + 1) * 4);
+    put(p.init, M1 * 4);
+    put(p.alpha, M1 * 8);
+    put(p.eel, M1 * 8);
+    put(p.mw, M1 * 8);
+    put(p.gene, ((size_t)n_genes + 1) * 4);
+    put(p.samples, (size_t)n_chains * 4);
+    put(p.seeds, (size_t)n_chains * 4);
+    put(p.cv_off, (size_t)n_chains * 8);
+    p.head = at;
+    put(p.sync, (size_t)n_chains * sizeof(ChainSync));
+    put(p.slice_tot, (size_t)n_chains * kBatchMaxWorkers * 4);
+    put(p.acc, (size_t)n_chains * (4 * M1 + (size_t)n_genes) * 8);
+    p.zero_end = at;
+    put(p.cv, (size_t)n_samples * M1 * 4);
+    p.total = at;
+    return p;
+}
+}  // namespace
+
+}  // namespace rsem_b200
+
+struct rsem_b200_gibbs_batch {
+    struct Slot {
+        bool live = false, ran = false;
+        void* block = nullptr;
+        uint64_t bytes = 0;
+        int n_chains = 0, n_samples = 0;
+        uint64_t cost = 0;                 // reads x sweeps of its longest chain: the claim order
+        std::vector<int32_t> chain_samples;
+        rsem_b200::PArgs a{};              // device pointers into the block; scratch pointers are the team's
+        size_t sync_off = 0, acc_off = 0, cv_off = 0;
+    };
+    rsem_b200_ctx* ctx = nullptr;
+    uint64_t capacity = 0, used = 0;
+    int k = 2;
+    int M = -1, n_genes = -1;
+    std::vector<Slot> slots;
+};
+
+namespace rsem_b200 {
+
+int gibbs_batch_create(rsem_b200_ctx* c, uint64_t capacity, int worker_ctas, rsem_b200_gibbs_batch** out) {
+    if (worker_ctas < 0 || worker_ctas > kBatchMaxWorkers) { set_error("gibbs_batch_create: worker_ctas must be 0..8"); return RSEM_B200_ERR_ARG; }
+    RB_CUDA(cudaSetDevice(c->device));
+    if (capacity == 0) {   // half of the device memory that is free now
+        size_t free_b = 0, total_b = 0;
+        RB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        capacity = free_b / 2;
+    }
+    auto* b = new rsem_b200_gibbs_batch();
+    b->ctx = c;
+    b->capacity = capacity;
+    b->k = worker_ctas ? worker_ctas : kBatchDefaultWorkers;
+    *out = b;
+    return 0;
+}
+
+void gibbs_batch_clear(rsem_b200_gibbs_batch* b) {
+    cudaSetDevice(b->ctx->device);
+    for (auto& s : b->slots)
+        if (s.live) cudaFreeAsync(s.block, b->ctx->stream);
+    cudaStreamSynchronize(b->ctx->stream);
+    b->slots.clear();
+    b->used = 0;
+    b->M = b->n_genes = -1;
+}
+
+void gibbs_batch_destroy(rsem_b200_gibbs_batch* b) {
+    gibbs_batch_clear(b);
+    delete b;
+}
+
+int gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes, int32_t n_samples, int32_t n_chains,
+                             uint64_t* bytes) {
+    if (N1 < RSEM_B200_GIBBS_BATCH_MIN_READS || N1 > RSEM_B200_GIBBS_BATCH_MAX_READS) {
+        set_error("the sample is outside the Gibbs batch's size rule (1248 <= N1 <= 2^19 reads): run it with "
+                  "rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains");
+        return RSEM_B200_ERR_UNSUPPORTED;
+    }
+    *bytes = gparts(N1, E, M, n_genes, n_samples, n_chains).total;
+    return 0;
+}
+
+int gibbs_batch_add(rsem_b200_gibbs_batch* b, uint64_t N1, uint64_t E, const uint64_t* row_ptr, const int32_t* sid,
+                    const double* conprb, const rsem_b200_gibbs_params* p, int32_t* slot_out) {
+    rsem_b200_ctx* c = b->ctx;
+    const int M = p->M, nc = p->n_chains;
+    if (b->M >= 0 && (M != b->M || p->n_genes != b->n_genes)) {
+        set_error("gibbs_batch_add: every sample of a batch has the M and n_genes of the first");
+        return RSEM_B200_ERR_ARG;
+    }
+    int64_t n_samples = 0;
+    uint64_t longest = 0;
+    for (int t = 0; t < nc; ++t) {
+        if (p->chain_samples[t] < 1) { set_error("gibbs_batch_add: every chain keeps at least one sample"); return RSEM_B200_ERR_ARG; }
+        n_samples += p->chain_samples[t];
+        longest = std::max<uint64_t>(longest, (uint64_t)p->burnin + 2 + (uint64_t)(p->chain_samples[t] - 1) * p->gap);
+    }
+    uint64_t bytes = 0;
+    if (int rc = gibbs_batch_sample_bytes(N1, E, M, p->n_genes, (int32_t)n_samples, nc, &bytes)) return rc;
+    if (b->used + bytes > b->capacity) {
+        set_error("the Gibbs batch arena is full");
+        return RSEM_B200_ERR_FULL;
+    }
+    GibbsLayout L;
+    if (int rc = gibbs_layout(row_ptr, sid, N1, M, L)) return rc;
+    // a row without entries has nothing to draw from (as gibbs_run refuses it)
+    if (L.empty_row) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
+    const GParts q = gparts(N1, E, M, p->n_genes, (int)n_samples, nc);
+    const size_t M1 = (size_t)M + 1;
+    std::vector<unsigned char> img(q.head, 0);
+    auto put = [&](size_t off, const void* src, size_t n) { if (n) memcpy(img.data() + off, src, n); };
+    put(q.order, L.order.data(), N1 * 4);
+    put(q.p_off, L.p_off.data(), (N1 + 1) * 8);
+    put(q.p_sid, L.p_sid.data(), E * 4);
+    {
+        double* pc = reinterpret_cast<double*>(img.data() + q.p_con);
+        for (uint64_t r = 0; r < N1; ++r) {
+            const uint64_t src = row_ptr[L.order[r]], n = row_ptr[L.order[r] + 1] - src;
+            memcpy(pc + L.p_off[r], conprb + src, n * 8);
+        }
+    }
+    put(q.seg_start, L.seg_start.data(), L.seg_start.size() * 4);
+    put(q.seg_ntr, L.seg_ntr.data(), L.seg_ntr.size() * 4);
+    put(q.seg_tid_off, L.seg_tid_off.data(), L.seg_tid_off.size() * 4);
+    put(q.comp_tids, L.comp_tids.data(), L.comp_tids.size() * 4);
+    put(q.init, p->init_counts, M1 * 4);
+    put(q.alpha, p->pseudo_counts, M1 * 8);
+    put(q.eel, p->eel, M1 * 8);
+    put(q.mw, p->mw, M1 * 8);
+    put(q.gene, p->gene_start, ((size_t)p->n_genes + 1) * 4);
+    put(q.samples, p->chain_samples, (size_t)nc * 4);
+    put(q.seeds, p->chain_seeds, (size_t)nc * 4);
+    {
+        long long* off = reinterpret_cast<long long*>(img.data() + q.cv_off);
+        long long at = 0;
+        for (int t = 0; t < nc; ++t) { off[t] = at; at += p->chain_samples[t]; }
+    }
+    RB_CUDA(cudaSetDevice(c->device));
+    void* block = nullptr;
+    RB_CUDA(cudaMallocAsync(&block, q.total, c->stream));
+    RB_CUDA(cudaMemcpyAsync(block, img.data(), q.head, cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(block) + q.head, 0, q.zero_end - q.head, c->stream));   // sync, slice totals, sums
+    RB_CUDA(cudaStreamSynchronize(c->stream));   // img goes out of scope
+
+    int slot = -1;
+    for (size_t i = 0; i < b->slots.size(); ++i) if (!b->slots[i].live) { slot = (int)i; break; }
+    if (slot < 0) { slot = (int)b->slots.size(); b->slots.emplace_back(); }
+    auto& s = b->slots[slot];
+    s = rsem_b200_gibbs_batch::Slot{};
+    s.live = true;
+    s.block = block;
+    s.bytes = bytes;
+    s.n_chains = nc;
+    s.n_samples = (int)n_samples;
+    s.cost = longest * N1;
+    s.chain_samples.assign(p->chain_samples, p->chain_samples + nc);
+    s.sync_off = q.sync; s.acc_off = q.acc; s.cv_off = q.cv;
+    unsigned char* base = static_cast<unsigned char*>(block);
+    PArgs& a = s.a;
+    a.N1 = N1;
+    a.order = reinterpret_cast<const int*>(base + q.order);
+    a.p_off = reinterpret_cast<const unsigned long long*>(base + q.p_off);
+    a.p_sid = reinterpret_cast<const int*>(base + q.p_sid);
+    a.p_con = reinterpret_cast<const double*>(base + q.p_con);
+    a.seg_start = reinterpret_cast<const int*>(base + q.seg_start);
+    a.seg_ntr = reinterpret_cast<const int*>(base + q.seg_ntr);
+    a.seg_tid_off = reinterpret_cast<const int*>(base + q.seg_tid_off);
+    a.comp_tids = reinterpret_cast<const int*>(base + q.comp_tids);
+    a.n_segs = L.n_segs;
+    a.fast_rows = 1;
+    a.M = M; a.burnin = p->burnin; a.gap = p->gap; a.n_genes = p->n_genes; a.n_chains = nc;
+    a.ctas_per_chain = b->k;
+    a.chain_samples = reinterpret_cast<const int*>(base + q.samples);
+    a.chain_seeds = reinterpret_cast<const unsigned*>(base + q.seeds);
+    a.chain_cv_offset = reinterpret_cast<const long long*>(base + q.cv_off);
+    a.n0 = p->n0; a.totc = p->totc;
+    a.init_counts = reinterpret_cast<const int*>(base + q.init);
+    a.alpha = reinterpret_cast<const double*>(base + q.alpha);
+    a.eel = reinterpret_cast<const double*>(base + q.eel);
+    a.mw = reinterpret_cast<const double*>(base + q.mw);
+    a.gene_start = reinterpret_cast<const int*>(base + q.gene);
+    a.slice_tot = reinterpret_cast<int*>(base + q.slice_tot);
+    a.n_words = (unsigned)((N1 + 31) / 32);
+    a.sync = reinterpret_cast<ChainSync*>(base + q.sync);
+    a.count_vectors = reinterpret_cast<int*>(base + q.cv);
+    a.acc = reinterpret_cast<double*>(base + q.acc);
+    b->used += bytes;
+    b->M = M;
+    b->n_genes = p->n_genes;
+    *slot_out = slot;
+    return 0;
+}
+
+int gibbs_batch_run(rsem_b200_gibbs_batch* b, rsem_b200_gibbs_batch_stats* stats) {
+    rsem_b200_ctx* c = b->ctx;
+    if (stats) *stats = rsem_b200_gibbs_batch_stats{0, b->k, 0, 0, 0, 0};
+    std::vector<int> run;
+    for (size_t i = 0; i < b->slots.size(); ++i)
+        if (b->slots[i].live && !b->slots[i].ran) run.push_back((int)i);
+    if (run.empty()) return 0;
+    RB_CUDA(cudaSetDevice(c->device));
+    std::vector<PArgs> args;
+    std::vector<int2> jobs;
+    uint64_t n1_max = 0;
+    for (size_t r = 0; r < run.size(); ++r) {
+        const auto& s = b->slots[run[r]];
+        args.push_back(s.a);
+        n1_max = std::max<uint64_t>(n1_max, s.a.N1);
+        for (int t = 0; t < s.n_chains; ++t) jobs.push_back(make_int2((int)r, t));
+    }
+    // largest first: reads x sweeps of the chain, so that the long jobs start first and the short ones fill in behind them
+    auto cost = [&](const int2& j) {
+        const PArgs& a = args[j.x];
+        return a.N1 * (uint64_t)(a.burnin + 2 + (uint64_t)(b->slots[run[j.x]].chain_samples[j.y] - 1) * a.gap);
+    };
+    std::stable_sort(jobs.begin(), jobs.end(), [&](const int2& x, const int2& y) { return cost(x) > cost(y); });
+    int per_sm = 0;
+    RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gibbs_batch_kernel, kPThreads, 0));
+    const int resident = std::max(1, per_sm) * c->sm_count;
+    if (resident < b->k + 1) { set_error("gibbs_batch_run: a team does not fit the device"); return RSEM_B200_ERR_UNSUPPORTED; }
+    const int teams = std::min<int>((int)jobs.size(), resident / (b->k + 1));
+    const int M1 = b->M + 1;
+    const unsigned w_max = (unsigned)((n1_max + 31) / 32);
+
+    BArgs ba{};
+    ba.n_jobs = (unsigned)jobs.size();
+    ba.k = (unsigned)b->k;
+    ba.n1_max = n1_max;
+    ba.w_max = w_max;
+    ba.M1 = M1;
+    void* scratch = nullptr;
+    const size_t per_team[] = {(size_t)M1 * 4, (size_t)M1 * 4, 2 * n1_max * 4, 2 * n1_max * 4, 4 * (size_t)w_max * 4,
+                               (size_t)w_max * 4, 2 * (size_t)M1 * 8};
+    size_t off[8] = {0};
+    for (int i = 0; i < 7; ++i) off[i + 1] = off[i] + align_up(per_team[i] * teams);
+    const size_t head = align_up(args.size() * sizeof(PArgs)) + align_up(jobs.size() * sizeof(int2)) + 256 + align_up(teams * 8ull);
+    RB_CUDA(cudaMallocAsync(&scratch, off[7] + head, c->stream));
+    unsigned char* sb = static_cast<unsigned char*>(scratch);
+    ba.counts = reinterpret_cast<int*>(sb + off[0]);
+    ba.counts_start = reinterpret_cast<int*>(sb + off[1]);
+    ba.z = reinterpret_cast<int*>(sb + off[2]);
+    ba.ubuf = reinterpret_cast<unsigned*>(sb + off[3]);
+    ba.flips = reinterpret_cast<unsigned*>(sb + off[4]);
+    ba.pre = reinterpret_cast<int*>(sb + off[5]);
+    ba.theta_tmp = reinterpret_cast<double*>(sb + off[6]);
+    unsigned char* hp = sb + off[7];
+    ba.samples = reinterpret_cast<const PArgs*>(hp);
+    hp += align_up(args.size() * sizeof(PArgs));
+    ba.jobs = reinterpret_cast<const int2*>(hp);
+    hp += align_up(jobs.size() * sizeof(int2));
+    ba.next_job = reinterpret_cast<unsigned*>(hp);
+    ba.mailbox = reinterpret_cast<unsigned long long*>(hp + 256);
+    int rc = 0;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    auto fail = [&](cudaError_t e, const char* what) {
+        if (!rc) rc = cuda_fail(e, what, __FILE__, __LINE__);
+    };
+    cudaError_t e = cudaMemcpyAsync((void*)ba.samples, args.data(), args.size() * sizeof(PArgs), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync((void*)ba.jobs, jobs.data(), jobs.size() * sizeof(int2), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(hp, 0, 256 + align_up(teams * 8ull), c->stream);
+    if (e == cudaSuccess) e = cudaEventCreate(&ev0);
+    if (e == cudaSuccess) e = cudaEventCreate(&ev1);
+    if (e == cudaSuccess) e = cudaEventRecord(ev0, c->stream);
+    if (e == cudaSuccess) {
+        void* kargs[] = {(void*)&ba};
+        e = cudaLaunchCooperativeKernel((void*)gibbs_batch_kernel, dim3(teams * (b->k + 1)), dim3(kPThreads), kargs, 0, c->stream);
+        c->launches++;
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ev1, c->stream);
+    if (e != cudaSuccess) fail(e, "gibbs_batch_kernel launch");
+    cudaFreeAsync(scratch, c->stream);
+    e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) fail(e, "cudaStreamSynchronize");
+    float ms = 0;
+    if (!rc && cudaEventElapsedTime(&ms, ev0, ev1) != cudaSuccess) ms = 0;
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (rc) return rc;
+    bool err = false;
+    uint64_t chain_cyc = 0, sample_cyc = 0;
+    for (int i : run) {
+        auto& s = b->slots[i];
+        std::vector<ChainSync> sy(s.n_chains);
+        RB_CUDA(cudaMemcpy(sy.data(), static_cast<unsigned char*>(s.block) + s.sync_off, s.n_chains * sizeof(ChainSync),
+                           cudaMemcpyDeviceToHost));
+        for (const ChainSync& y : sy) {
+            err = err || y.err;
+            chain_cyc += y.prof[0] + y.prof[2] + y.prof[3];
+            sample_cyc += y.prof[3];
+        }
+        s.ran = true;
+    }
+    if (stats) *stats = rsem_b200_gibbs_batch_stats{ms, b->k, teams, (int64_t)jobs.size(), chain_cyc, sample_cyc};
+    if (err) {
+        set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
+        return RSEM_B200_ERR_ARG;
+    }
+    return 0;
+}
+
+int gibbs_batch_result(rsem_b200_gibbs_batch* b, int32_t slot, int32_t* count_vectors, double* chain_acc) {
+    if (slot < 0 || slot >= (int)b->slots.size() || !b->slots[slot].live) { set_error("no sample in this slot"); return RSEM_B200_ERR_ARG; }
+    const auto& s = b->slots[slot];
+    if (!s.ran) { set_error("gibbs_batch_result: the sample has not run yet"); return RSEM_B200_ERR_ARG; }
+    rsem_b200_ctx* c = b->ctx;
+    const size_t M1 = (size_t)b->M + 1, acc_per = 4 * M1 + (size_t)b->n_genes;
+    RB_CUDA(cudaSetDevice(c->device));
+    const unsigned char* base = static_cast<const unsigned char*>(s.block);
+    RB_CUDA(cudaMemcpyAsync(count_vectors, base + s.cv_off, (size_t)s.n_samples * M1 * 4, cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaMemcpyAsync(chain_acc, base + s.acc_off, (size_t)s.n_chains * acc_per * 8, cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
 }
 
 }  // namespace rsem_b200

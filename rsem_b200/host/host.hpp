@@ -189,6 +189,19 @@ void write_results_em(const std::string& ref_name, const std::string& imd_name, 
 void write_em_outputs(const std::string& refName, const std::string& imdName, const std::string& statName,
                       const RefData& refs, const std::vector<TranscriptInfo>& transcripts, const HostModel& model,
                       std::vector<double> theta, const std::vector<double>& counts, bool appendNames);
+// gibbs_sample.cpp: the per-sample stages of rsem-run-gibbs (also used by rsem-run-gibbs-batch)
+// load_omit_info / load_prior_info (Gibbs.cpp:152-194): init_counts (-1 = omitted), alpha and totc of a sample with N0 + N1
+// reads; returns "" or why imdName.omit or the prior file cannot be used.
+std::string gibbs_inputs(const std::string& imdName, int M, uint64_t N0, uint64_t N1, double pseudoC, const std::string* fprior,
+                         std::vector<int32_t>& init_counts, std::vector<double>& alpha, double& totc);
+// imdName.countvectors<t>, one per chain (Gibbs.cpp:257-262); cvs holds the chains' vectors in chain order
+void write_countvectors(const std::string& imdName, int M, const std::vector<int32_t>& chain_samples, const int32_t* cvs);
+// release() (Gibbs.cpp:399-422): means and unbiased variances from the sums of all chains and the kept count vectors,
+// then imdName.iso_res / gene_res (and the allele file) by write_results_gibbs
+void write_gibbs_results(const std::string& refName, const std::string& imdName, int M, int NSAMPLES, const std::vector<int>& gi,
+                         bool alleleS, const std::vector<int>& ta, const int32_t* cvs, const std::vector<double>& sum_c,
+                         const std::vector<double>& sum_c2, const std::vector<double>& sum_tpm, const std::vector<double>& sum_fpkm,
+                         const std::vector<double>& sum_g2);
 void write_results_gibbs(const std::string& ref_name, const std::string& imd_name, int M, const std::vector<double>& pme_c,
                          const std::vector<double>& pme_fpkm, const std::vector<double>& pme_tpm,
                          const std::vector<double>& pve_c, const std::vector<double>& pve_c_genes,
