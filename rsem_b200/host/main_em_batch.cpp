@@ -9,7 +9,9 @@
 // 11 on, its frozen rounds join a batch (K12, rsem_b200_batch_*) that converges every sample in it with one kernel
 // launch per few dozen rounds.  A sample outside the batch layout (rsem_b200_batch_sample_bytes) finishes on the context
 // with rsem_b200_em_rounds right after its round 10.  When the batch arena is full, the samples in it are run to the end
-// and written before the next one is added.  Standard output has one block per sample, in manifest order.
+// and written before the next one is added; a sample that still does not fit then finishes on the context.
+// RSEM_B200_BATCH_ARENA_BYTES sets the arena's size (default, or 0: half of the device memory free at the start).
+// Standard output has one block per sample, in manifest order.
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
@@ -74,6 +76,11 @@ struct Timed {
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return v ? atoi(v) : dflt;
+}
+
+uint64_t env_bytes(const char* name) {   // 0 when unset
+    const char* v = getenv(name);
+    return v ? strtoull(v, nullptr, 10) : 0;
 }
 
 std::string round_line(int round, const rsem_b200_round_stats& s) {
@@ -178,7 +185,8 @@ int main(int argc, char* argv[]) {
     check_rc(rsem_b200_upload_refs(ctx, M, refs.seq_off.data(), refs.seq.data(), refs.full_len.data(), refs.tot_len.data(),
                                    refs.mask_off.data(), refs.mask_words.data()), "upload_refs");
     rsem_b200_batch* batch = nullptr;
-    check_rc(rsem_b200_batch_create(ctx, 0, &batch), "batch_create");
+    check_rc(rsem_b200_batch_create(ctx, env_bytes("RSEM_B200_BATCH_ARENA_BYTES"), &batch), "batch_create");
+    int n_batched = 0, n_single = 0, n_full = 0;   // samples whose frozen rounds ran in the batch / on the context; full arenas
 
     Phases ph;
     std::vector<std::string> block(lines.size());
@@ -337,15 +345,18 @@ int main(int argc, char* argv[]) {
             int rc = rsem_b200_batch_add(batch, hits.N, hits.H, M, hits.row_ptr.data(), hits.sid.data(), p->conprb.data(),
                                          p->ncpv.data(), theta.data(), (double)l.N0, ROUND + 1, MIN_ROUND, MAX_ROUND, &slot);
             if (rc == RSEM_B200_ERR_FULL) {
+                ++n_full;
                 drain();
                 rc = rsem_b200_batch_add(batch, hits.N, hits.H, M, hits.row_ptr.data(), hits.sid.data(), p->conprb.data(),
                                          p->ncpv.data(), theta.data(), (double)l.N0, ROUND + 1, MIN_ROUND, MAX_ROUND, &slot);
             }
             if (rc == 0) {
+                ++n_batched;
                 in_batch[slot] = std::move(p);
                 continue;
             }
             if (rc != RSEM_B200_ERR_UNSUPPORTED && rc != RSEM_B200_ERR_FULL) check_rc(rc, "batch_add");
+            ++n_single;
             std::vector<rsem_b200_round_stats> cs(32);
             Timed tk{ph.frozen};
             while (keep_going) {
@@ -374,7 +385,9 @@ int main(int argc, char* argv[]) {
     uint64_t k12_rounds = 0;
     check_rc(rsem_b200_batch_timing(batch, &k12_ms, &k12_rounds), "batch_timing");
     if (getenv("RSEM_B200_TIMING")) {
-        fprintf(stderr, "rsem-run-em-batch timing: K12 %.3f ms over %llu sample-rounds\n", k12_ms, (unsigned long long)k12_rounds);
+        fprintf(stderr, "rsem-run-em-batch timing: %d samples in the batch, %d on the single-sample path; K12 %.3f ms over %llu "
+                "sample-rounds\n", n_batched, n_single, k12_ms, (unsigned long long)k12_rounds);
+        fprintf(stderr, "rsem-run-em-batch timing: arena full %d times\n", n_full);
         fprintf(stderr, "rsem-run-em-batch timing: load %.3f s, model rounds %.3f s, frozen rounds %.3f s, final pass %.3f s, "
                 "writers %.3f s\n", ph.load, ph.model, ph.frozen, ph.final, ph.write);
     }

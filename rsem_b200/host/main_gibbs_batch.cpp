@@ -7,8 +7,9 @@
 // and each line gets the files `rsem-run-gibbs refName <line>` writes.  One CUDA context (RSEM_B200_DEVICE) serves the whole
 // run.  A sample of 1248 .. 2^19 reads joins a Gibbs batch (K13, rsem_b200_gibbs_batch_*), which runs the chains of all its
 // samples in one launch; any other sample runs on the context with rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains, as in
-// rsem-run-gibbs.  When the batch arena is full, the samples in it are run and written before the next one is added.
-// Standard output has one block per sample, in manifest order.
+// rsem-run-gibbs.  When the batch arena is full, the samples in it are run and written before the next one is added; a
+// sample that still does not fit then runs on the context.  RSEM_B200_BATCH_ARENA_BYTES sets the arena's size
+// (default, or 0: half of the device memory free at the start).  Standard output has one block per sample, in manifest order.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -137,7 +138,7 @@ struct Phases {
     double load = 0, device = 0, copy = 0, write = 0;
     double k13_ms = 0;
     uint64_t chain_cycles = 0, sample_cycles = 0, jobs = 0;
-    int teams = 0, workers = 0, batched = 0, single = 0;
+    int teams = 0, workers = 0, batched = 0, single = 0, full = 0;
 };
 
 }  // namespace
@@ -243,7 +244,8 @@ int main(int argc, char* argv[]) {
         ctx = r.ctx;
     }
     rsem_b200_gibbs_batch* batch = nullptr;
-    check_rc(rsem_b200_gibbs_batch_create(ctx, 0, 0, &batch), "gibbs_batch_create");
+    const char* arena = getenv("RSEM_B200_BATCH_ARENA_BYTES");
+    check_rc(rsem_b200_gibbs_batch_create(ctx, arena ? strtoull(arena, nullptr, 10) : 0, 0, &batch), "gibbs_batch_create");
 
     // the samples in the batch run in one launch; their outputs are copied back one by one and written on worker threads
     std::map<int32_t, std::unique_ptr<Sample>> in_batch;
@@ -317,6 +319,7 @@ int main(int argc, char* argv[]) {
         int rc = rsem_b200_gibbs_batch_add(batch, s->N1, s->sid.size(), s->row_ptr.data(), s->sid.data(), s->conprb.data(), &gp, &slot);
         ph.load += now_s() - t_load;
         if (rc == RSEM_B200_ERR_FULL) {
+            ++ph.full;
             drain();
             const double t0 = now_s();
             rc = rsem_b200_gibbs_batch_add(batch, s->N1, s->sid.size(), s->row_ptr.data(), s->sid.data(), s->conprb.data(), &gp, &slot);
@@ -362,6 +365,7 @@ int main(int argc, char* argv[]) {
                 ph.chain_cycles ? (double)ph.sample_cycles / (double)ph.chain_cycles : 0.0);
         fprintf(stderr, "rsem-run-gibbs-batch timing: load+components %.3f s, device %.3f s, copies back %.3f s, writers %.3f s "
                 "(thread seconds), count-vector text %llu bytes\n", ph.load, ph.device, ph.copy, ph.write, (unsigned long long)cv_bytes);
+        fprintf(stderr, "rsem-run-gibbs-batch timing: arena full %d times\n", ph.full);
     }
     rsem_b200_gibbs_batch_destroy(batch);
     rsem_b200_ctx_destroy(ctx);
