@@ -98,6 +98,8 @@ typedef struct rsem_b200_round_stats {
 int rsem_b200_version(void);
 const char* rsem_b200_last_error(void);
 int rsem_b200_device_count(int* n_devices);
+/* bytes of device memory free on `device` now; the batch executables size their arenas from it */
+int rsem_b200_device_free_bytes(int device, uint64_t* free_bytes);
 
 /* One context per GPU (one host thread or process per context). */
 int rsem_b200_ctx_create(int device, rsem_b200_ctx** out);

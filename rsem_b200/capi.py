@@ -129,7 +129,8 @@ def _arr(a, dtype) -> Optional[np.ndarray]:
 
 # every symbol include/rsem_b200.h declares (tests check that the .so exports all of them)
 SYMBOLS = [
-    "rsem_b200_version", "rsem_b200_last_error", "rsem_b200_device_count", "rsem_b200_ctx_create",
+    "rsem_b200_version", "rsem_b200_last_error", "rsem_b200_device_count", "rsem_b200_device_free_bytes",
+    "rsem_b200_ctx_create",
     "rsem_b200_ctx_destroy", "rsem_b200_ctx_set_stream", "rsem_b200_ctx_sync", "rsem_b200_ctx_device_bytes",
     "rsem_b200_comm_unique_id", "rsem_b200_comm_init", "rsem_b200_upload_hits", "rsem_b200_upload_conprb",
     "rsem_b200_download_conprb", "rsem_b200_adopt_device_matrix", "rsem_b200_upload_reads", "rsem_b200_upload_refs",

@@ -369,7 +369,7 @@ int launch(rsem_b200_batch* b, const std::vector<BatchDesc>& descs, int rounds) 
     for (const auto& d : descs) max_m1 = std::max(max_m1, d.m1);
     const size_t smem = kThetaOffset + (size_t)max_m1 * sizeof(double);
     auto kern = k12_kernel<FINAL>;
-    RB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RB_CUDA(raise_dyn_smem((const void*)kern, smem));
     int per_sm = 0;
     RB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
     const int grid = std::max(1, std::min<int>((int)descs.size(), std::max(per_sm, 1) * c->sm_count));

@@ -4,6 +4,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <map>
+#include <mutex>
 
 #include "common.cuh"
 
@@ -18,6 +20,20 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line) {
     snprintf(buf, sizeof buf, "CUDA error %d (%s) at %s:%d: %s", (int)e, cudaGetErrorString(e), file, line, what);
     g_last_error = buf;
     return RSEM_B200_ERR_CUDA;
+}
+
+cudaError_t raise_dyn_smem(const void* kern, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> limit;   // (device, kernel) -> limit set so far
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> g(mu);
+    size_t& cur = limit[{dev, kern}];
+    if (bytes <= cur) return cudaSuccess;
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
 }
 
 // ---- device block cache ---------------------------------------------------------------------------------------------
@@ -225,6 +241,18 @@ int rsem_b200_device_count(int* n) {
     RB_ARG(n, "n_devices is NULL");
     *n = 0;
     RB_CUDA(cudaGetDeviceCount(n));
+    return 0;
+}
+
+int rsem_b200_device_free_bytes(int device, uint64_t* free_bytes) {
+    RB_ARG(free_bytes, "free_bytes is NULL");
+    int n = 0;
+    RB_CUDA(cudaGetDeviceCount(&n));
+    RB_ARG(device >= 0 && device < n, "device index out of range");
+    RB_CUDA(cudaSetDevice(device));
+    size_t free_b = 0, total_b = 0;
+    RB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    *free_bytes = free_b;
     return 0;
 }
 

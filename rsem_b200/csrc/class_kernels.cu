@@ -1184,10 +1184,10 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         constexpr int W = 15, U = 2;
         const size_t smem = sizeof(ClassSmem<W>);
         if (ctx->profiling) {
-            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            RB_CUDA(raise_dyn_smem((const void*)estep_class_kernel<W, U, false, true>, smem));
             estep_class_kernel<W, U, false, true><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         } else {
-            RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            RB_CUDA(raise_dyn_smem((const void*)estep_class_kernel<W, U, false, false>, smem));
             estep_class_kernel<W, U, false, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         }
         RB_CUDA(cudaGetLastError());
@@ -1201,7 +1201,7 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
         constexpr int W = 11, U = 2;
         const size_t smem = sizeof(ClassSmem<W>);
-        RB_CUDA(cudaFuncSetAttribute(estep_class_kernel<W, U, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        RB_CUDA(raise_dyn_smem((const void*)estep_class_kernel<W, U, true, false>, smem));
         estep_class_kernel<W, U, true, false><<<grid, (W + 1) * 32, smem, ctx->stream>>>(a);
         RB_CUDA(cudaGetLastError());
         ctx->launches++;

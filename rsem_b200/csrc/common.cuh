@@ -18,6 +18,10 @@ constexpr double kEpsilon = 1e-300;
 
 void set_error(const std::string& msg);
 int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
+// cudaFuncSetAttribute(kern, MaxDynamicSharedMemorySize, bytes) on the current device, but never lowering the limit:
+// host threads may launch one kernel on one device side by side (the lanes of rsem-run-em-batch), and a limit set to
+// each launch's own size could be lowered by another thread between a set and its launch.
+cudaError_t raise_dyn_smem(const void* kern, size_t bytes);
 
 #define RB_CUDA(call)                                                       \
     do {                                                                    \

@@ -522,7 +522,7 @@ template <int G, bool WP>
 int launch_rows(rsem_b200_ctx* ctx, const EstepArgs& a) {
     auto kern = estep_rows_kernel<G, WP>;
     const size_t smem = sizeof(RowSmem);
-    RB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RB_CUDA(raise_dyn_smem((const void*)kern, smem));
     const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
     kern<<<grid, kThreads, smem, ctx->stream>>>(a);
     RB_CUDA(cudaGetLastError());

@@ -976,7 +976,7 @@ int launch_conprb_g(rsem_b200_ctx* c, const ModelArgs& a, unsigned grid, size_t 
     do {                                                                                                     \
         if (smem) {                                                                                          \
             auto k = conprb_kernel<G, Q, P, true>;                                                           \
-            if (smem > 48 * 1024) RB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            if (smem > 48 * 1024) RB_CUDA(raise_dyn_smem((const void*)k, smem));                             \
             k<<<grid, kBlock, smem, c->stream>>>(a);                                                         \
         } else {                                                                                             \
             conprb_kernel<G, Q, P, false><<<grid, kBlock, 0, c->stream>>>(a);                                \
@@ -998,7 +998,7 @@ int launch_update_q(rsem_b200_ctx* c, const ModelArgs& a) {
     const size_t per_warp = (size_t)a.q_rows * 30 * sizeof(double);
     const int warps = (int)std::max<size_t>(1, std::min<size_t>(kQMaxWarps, (size_t)(200 * 1024) / per_warp));
     const size_t smem = per_warp * warps;
-    RB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RB_CUDA(raise_dyn_smem((const void*)k, smem));
     k<<<c->sm_count, warps * 32, smem, c->stream>>>(a);
     RB_CUDA(cudaGetLastError());
     c->launches++;
@@ -1011,7 +1011,7 @@ int launch_update_coop(rsem_b200_ctx* c, const ModelArgs& a) {
     const size_t per_warp = HASQ ? (size_t)a.q_rows * 30 * sizeof(double) : 0;
     const int warps = HASQ ? (int)std::max<size_t>(1, std::min<size_t>(kQMaxWarps, (size_t)(200 * 1024) / per_warp)) : kQMaxWarps;
     const size_t smem = per_warp * warps;
-    if (smem > 48 * 1024) RB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024) RB_CUDA(raise_dyn_smem((const void*)k, smem));
     k<<<c->sm_count * (HASQ ? 1 : 2), warps * 32, smem, c->stream>>>(a);
     RB_CUDA(cudaGetLastError());
     c->launches++;

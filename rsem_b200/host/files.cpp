@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
+#include <stdexcept>
 #include <set>
 #include <thread>
 
@@ -29,7 +30,15 @@ void parallel_ranges(size_t n, int parts, const std::function<void(size_t, size_
     for (auto& th : pool) th.join();
 }
 
+namespace {
+thread_local bool t_die_throws = false;
+}
+
+DieThrows::DieThrows(bool on) : prev(t_die_throws) { t_die_throws = on; }
+DieThrows::~DieThrows() { t_die_throws = prev; }
+
 void die(const std::string& msg) {
+    if (t_die_throws) throw std::runtime_error(msg);
     fprintf(stderr, "%s\n", msg.c_str());
     exit(-1);
 }
@@ -88,6 +97,72 @@ std::vector<int> gpu_devices() {
         devices.assign(1, one ? atoi(one) : devices.empty() ? 0 : devices[0]);
     }
     return devices;
+}
+
+LaneContexts open_lanes(const std::vector<int>& devices) {
+    const size_t n = devices.size();
+    LaneContexts out;
+    out.ctx.assign(n, nullptr);
+    out.arena.assign(n, 0);
+    const char* e = getenv("RSEM_B200_BATCH_ARENA_BYTES");
+    const uint64_t set = e ? strtoull(e, nullptr, 10) : 0;   // 0 is the default, as unset
+    out.arena.assign(n, set);
+    const bool share = n > 1 && set == 0;
+    std::vector<std::string> err(n);
+    std::vector<int> distinct;
+    for (int d : devices)
+        if (std::find(distinct.begin(), distinct.end(), d) == distinct.end()) distinct.push_back(d);
+    // per device: its free memory, then the contexts of its lanes; the devices side by side
+    auto open_device = [&](int d) {
+        std::vector<size_t> mine;
+        for (size_t k = 0; k < n; ++k)
+            if (devices[k] == d) mine.push_back(k);
+        const std::string where = n > 1 ? "device " + std::to_string(d) + ": " : "";
+        if (share) {
+            uint64_t free_b = 0;
+            if (rsem_b200_device_free_bytes(d, &free_b) != 0) {
+                err[mine[0]] = "rsem_b200: " + where + "device_free_bytes failed: " + rsem_b200_last_error();
+                return;
+            }
+            for (size_t k : mine) out.arena[k] = free_b / 2 / mine.size();
+        }
+        for (size_t k : mine)
+            if (rsem_b200_ctx_create(d, &out.ctx[k]) != 0) {
+                err[k] = "rsem_b200: " + where + "ctx_create failed: " + rsem_b200_last_error();
+                return;
+            }
+    };
+    {
+        std::vector<std::thread> pool;
+        for (size_t j = 1; j < distinct.size(); ++j) pool.emplace_back(open_device, distinct[j]);
+        open_device(distinct[0]);
+        for (auto& th : pool) th.join();
+    }
+    for (const std::string& m : err)
+        if (!m.empty()) {
+            out.err = m;
+            break;
+        }
+    return out;
+}
+
+size_t Claims::next() {
+    if (failed_) return n_;
+    return std::min(n_, i_.fetch_add(1));
+}
+
+void Claims::fail(const std::string& msg) {
+    std::lock_guard<std::mutex> g(mu_);
+    if (failed_) return;
+    msg_ = msg;
+    failed_ = true;
+}
+
+bool Claims::failed() { return failed_; }
+
+std::string Claims::message() {
+    std::lock_guard<std::mutex> g(mu_);
+    return msg_;
 }
 
 namespace {
@@ -174,8 +249,7 @@ void load_refs(const std::string& path, bool with_seqs, RefData& r) {
             for (long long k = 0; k < totLen; ++k) {
                 int8_t code = g_code[(unsigned char)b[k]];
                 if (code < 0) {
-                    fprintf(stderr, "Found unknown sequence letter %c at function get_base_id!\n", b[k]);
-                    exit(-1);
+                    die(std::string("Found unknown sequence letter ") + b[k] + " at function get_base_id!");
                 }
                 r.seq[at + k] = (uint8_t)code;
             }
@@ -200,7 +274,7 @@ void load_refs(const std::string& path, bool with_seqs, RefData& r) {
 // ---- ref.ti ---------------------------------------------------------------------------------------
 void load_transcripts(const std::string& path, std::vector<TranscriptInfo>& out, int* type_out) {
     std::ifstream fin(path.c_str());
-    if (!fin.is_open()) { fprintf(stderr, "Cannot open %s! It may not exist.\n", path.c_str()); exit(-1); }
+    if (!fin.is_open()) die("Cannot open " + path + "! It may not exist.");
     int M, type;
     std::string line;
     fin >> M >> type;
@@ -257,7 +331,7 @@ std::vector<int> map_bam_targets(const std::vector<std::string>& names, const st
 
 void load_groups(const std::string& path, std::vector<int>& starts) {
     FILE* fi = fopen(path.c_str(), "r");
-    if (!fi) { fprintf(stderr, "Cannot open %s! It may not exist.\n", path.c_str()); exit(-1); }
+    if (!fi) die("Cannot open " + path + "! It may not exist.");
     starts.clear();
     int pos;
     while (fscanf(fi, "%d", &pos) == 1) starts.push_back(pos);
@@ -339,7 +413,7 @@ void parse_reads(const std::string& imd, int tag, int read_type, bool has_polyA,
     std::vector<char> buf[2];
     for (int m = 0; m < s; ++m) {
         FILE* f = fopen(files[m].c_str(), "rb");
-        if (!f) { fprintf(stderr, "Cannot open %s! It may not exist.\n", files[m].c_str()); exit(-1); }
+        if (!f) die("Cannot open " + files[m] + "! It may not exist.");
         fclose(f);
         buf[m] = slurp(files[m]);
         if (!buf[m].empty() && buf[m].back() != '\n') buf[m].push_back('\n');

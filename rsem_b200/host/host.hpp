@@ -7,10 +7,12 @@
 // template classes, SoA read/hit stores instead of streams of objects.
 #pragma once
 
+#include <atomic>
 #include <cstdint>
 #include <cstdio>
 #include <functional>
 #include <map>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -349,5 +351,39 @@ uint32_t parse_seed(const char* s);  // digit-by-digit as EM.cpp:588-593
 // CUDA devices of a multi-GPU run: RSEM_B200_DEVICES=0,1,... in the order given; with at most one entry there,
 // RSEM_B200_DEVICE when it is set, else that entry, else device 0
 std::vector<int> gpu_devices();
+
+// ---- lanes of the batch executables: one host thread, context and batch arena per entry of gpu_devices() ----
+// While a DieThrows(true) lives on a thread, die() and check_rc() there throw std::runtime_error instead of ending the
+// process, so that a failing lane can be reported once the other lanes have stopped.
+struct DieThrows {
+    explicit DieThrows(bool on);
+    ~DieThrows();
+    bool prev;
+};
+// One context per entry of `devices`, created on host threads.  arena[k] is lane k's batch arena: RSEM_B200_BATCH_ARENA_BYTES
+// when it is set and not 0; else, with one entry, 0 (the batch's own default); else half of the device memory free before the first
+// context on the lane's device, divided by the entries naming that device.  err: the first device that could not be
+// opened, once every creation has returned (the caller ends the run).
+struct LaneContexts {
+    std::vector<rsem_b200_ctx*> ctx;
+    std::vector<uint64_t> arena;
+    std::string err;
+};
+LaneContexts open_lanes(const std::vector<int>& devices);
+// The manifest lines, handed to the lanes in manifest order; the first failure stops the handing out.
+class Claims {
+  public:
+    explicit Claims(size_t n) : n_(n) {}
+    size_t next();                          // n once every line is handed out or a lane has failed
+    void fail(const std::string& msg);      // keeps the first message
+    bool failed();
+    std::string message();
+  private:
+    const size_t n_;
+    std::atomic<size_t> i_{0};
+    std::atomic<bool> failed_{false};
+    std::mutex mu_;
+    std::string msg_;
+};
 
 }  // namespace host

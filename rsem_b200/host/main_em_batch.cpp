@@ -4,14 +4,20 @@
 //
 // Each non-empty manifest line is what rsem-run-em takes after read_type:
 //   sampleName imdName statName [-b samInpF has_fai [fai]] [--gibbs-out] [--sampling] [--seed s] [--append-names]
-// and each sample gets the files `rsem-run-em refName read_type <line> -p N` writes.  One CUDA context serves the whole
-// run; the reference is uploaded once.  A sample runs its model rounds 1-10 on the context as in rsem-run-em; from round
-// 11 on, its frozen rounds join a batch (K12, rsem_b200_batch_*) that converges every sample in it with one kernel
-// launch per few dozen rounds.  A sample outside the batch layout (rsem_b200_batch_sample_bytes) finishes on the context
-// with rsem_b200_em_rounds right after its round 10.  When the batch arena is full, the samples in it are run to the end
-// and written before the next one is added; a sample that still does not fit then finishes on the context.
-// RSEM_B200_BATCH_ARENA_BYTES sets the arena's size (default, or 0: half of the device memory free at the start).
-// Standard output has one block per sample, in manifest order.
+// and each sample gets the files `rsem-run-em refName read_type <line> -p N` writes.  A lane (a host thread, a CUDA context
+// holding the reference and a batch arena) takes the samples one by one.  A sample runs its model rounds 1-10 on the
+// lane's context as in rsem-run-em; from round 11 on, its frozen rounds join the lane's batch (K12, rsem_b200_batch_*) that
+// converges every sample in it with one kernel launch per few dozen rounds.  A sample outside the batch layout
+// (rsem_b200_batch_sample_bytes) finishes on the context with rsem_b200_em_rounds right after its round 10.  When the
+// batch arena is full, the samples in it are run to the end and written before the next one is added; a sample that
+// still does not fit then finishes on the context.
+// There is one lane on RSEM_B200_DEVICE (default 0), or one per entry of RSEM_B200_DEVICES=0,1,... when it lists more
+// than one; an entry may repeat a device (0,0 runs two lanes on device 0 side by side).  The lanes take the manifest lines
+// in manifest order from one counter; every sample runs on one CTA or on one context, so its files do not depend on the
+// lane that ran it.  RSEM_B200_BATCH_ARENA_BYTES sets each lane's arena (default, or 0: half of the device memory free at
+// the start, shared evenly by the lanes on one device).  The first failure of any lane ends the run with exit status
+// -1 once the other lanes have finished their current samples.  Standard output has one block per sample, in manifest
+// order.
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
@@ -21,6 +27,7 @@
 #include <map>
 #include <memory>
 #include <sstream>
+#include <thread>
 
 #include "host.hpp"
 
@@ -57,8 +64,7 @@ void usage() {
 }
 
 [[noreturn]] void refuse(const std::string& manifest, int no, const std::string& why) {
-    fprintf(stderr, "%s line %d: %s\n", manifest.c_str(), no, why.c_str());
-    exit(-1);
+    die(manifest + " line " + std::to_string(no) + ": " + why);
 }
 
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -76,11 +82,6 @@ struct Timed {
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
     return v ? atoi(v) : dflt;
-}
-
-uint64_t env_bytes(const char* name) {   // 0 when unset
-    const char* v = getenv(name);
-    return v ? strtoull(v, nullptr, 10) : 0;
 }
 
 std::string round_line(int round, const rsem_b200_round_stats& s) {
@@ -145,52 +146,46 @@ std::vector<Line> read_manifest(const std::string& path, int read_type) {
     return lines;
 }
 
-}  // namespace
-
-int main(int argc, char* argv[]) {
-    if (argc < 4) usage();
-    const time_t t_start = time(NULL);
-    const std::string refName = argv[1], manifest = argv[3];
-    const int read_type = atoi(argv[2]);
-    int nThreads = 1;
-    for (int i = 4; i < argc; ++i) {
-        if (!strcmp(argv[i], "-p") && i + 1 < argc) nThreads = atoi(argv[i + 1]);
-        if (!strcmp(argv[i], "-q")) g_verbose = false;
-    }
-    if (nThreads <= 0) die("Number of threads should be bigger than 0!");
-    g_io_threads = env_int("RSEM_B200_IO_THREADS", nThreads);
-    if (read_type < 0 || read_type > 3) { fprintf(stderr, "Unknown Read Type!\n"); exit(-1); }
-    std::vector<Line> lines = read_manifest(manifest, read_type);
-    const int MAX_ROUND = env_int("RSEM_MAX_ROUND", 10000), MIN_ROUND = env_int("RSEM_MIN_ROUND", 20);
-
-    struct CtxResult { int rc; rsem_b200_ctx* ctx; std::string err; };
-    std::future<CtxResult> ctx_future = std::async(std::launch::async, []() {
-        CtxResult r{0, nullptr, ""};
-        r.rc = rsem_b200_ctx_create(env_int("RSEM_B200_DEVICE", 0), &r.ctx);
-        if (r.rc != 0) r.err = rsem_b200_last_error();
-        return r;
-    });
+// what every lane reads
+struct Run {
+    std::string refName, manifest;
+    int read_type = 0, nThreads = 1, MAX_ROUND = 10000, MIN_ROUND = 20, M = 0, ti_type = 0;
+    std::vector<Line> lines;
     RefData refs;
-    load_refs(refName + ".seq", true, refs);
-    const int M = refs.M;
     std::vector<TranscriptInfo> transcripts;
-    int ti_type = 0;
-    load_transcripts(refName + ".ti", transcripts, &ti_type);
+    std::vector<std::string> block;   // standard output of each sample, written by the lane that took it
+};
+
+struct Lane {
+    int device = 0;
     rsem_b200_ctx* ctx = nullptr;
-    {
-        CtxResult r = ctx_future.get();
-        if (r.rc != 0) die("rsem_b200: ctx_create failed: " + r.err);
-        ctx = r.ctx;
-    }
+    uint64_t arena = 0;
+    rsem_b200_batch* batch = nullptr;
+    std::string where = "no sample yet";   // what the lane is working on, for the failure message
+    int n_batched = 0, n_single = 0, n_full = 0;   // samples whose frozen rounds ran in the batch / on the context; full arenas
+    double k12_ms = 0;
+    uint64_t k12_rounds = 0;
+    Phases ph;
+};
+
+// the samples a lane takes from `claims`, loaded, run and written on the lane's context and batch
+void run_lane(Run& R, Lane& L, Claims& claims) {
+    const std::vector<Line>& lines = R.lines;
+    const std::string& refName = R.refName;
+    const std::string& manifest = R.manifest;
+    const int read_type = R.read_type, M = R.M, MIN_ROUND = R.MIN_ROUND, MAX_ROUND = R.MAX_ROUND;
+    const RefData& refs = R.refs;
+    rsem_b200_ctx* ctx = L.ctx;
     check_rc(rsem_b200_upload_refs(ctx, M, refs.seq_off.data(), refs.seq.data(), refs.full_len.data(), refs.tot_len.data(),
                                    refs.mask_off.data(), refs.mask_words.data()), "upload_refs");
-    rsem_b200_batch* batch = nullptr;
-    check_rc(rsem_b200_batch_create(ctx, env_bytes("RSEM_B200_BATCH_ARENA_BYTES"), &batch), "batch_create");
-    int n_batched = 0, n_single = 0, n_full = 0;   // samples whose frozen rounds ran in the batch / on the context; full arenas
-
-    Phases ph;
-    std::vector<std::string> block(lines.size());
+    check_rc(rsem_b200_batch_create(ctx, L.arena, &L.batch), "batch_create");
+    rsem_b200_batch* batch = L.batch;
+    Phases& ph = L.ph;
+    std::vector<std::string>& block = R.block;
     auto say = [&](size_t i, const std::string& s) { if (g_verbose) block[i] += s; };
+    auto sample_at = [&](size_t i) {
+        return "sample " + lines[i].outName + " (" + manifest + " line " + std::to_string(lines[i].no) + ")";
+    };
 
     // outputs of a sample whose EM has ended: counts without N0, posteriors only with -b
     auto finish = [&](size_t i, const HitStore& hits, const HostModel& model, const std::vector<double>& theta,
@@ -203,10 +198,10 @@ int main(int argc, char* argv[]) {
                     l.outName.c_str(), MAX_ROUND);
         if (l.gibbsOut) write_ofg(l.imdName + ".ofg", M, l.N0, hits, conprb, ncpv);
         counts[0] += l.N0;
-        write_em_outputs(refName, l.imdName, l.statName, refs, transcripts, model, theta, counts, l.appendNames);
+        write_em_outputs(refName, l.imdName, l.statName, refs, R.transcripts, model, theta, counts, l.appendNames);
         if (l.genBam) {
-            write_posterior_bam(l.inpSamF, l.outName, read_type, l.bamSampling, l.hasSeed, l.seed, transcripts, ti_type,
-                                hits, post, post0, nThreads, false);
+            write_posterior_bam(l.inpSamF, l.outName, read_type, l.bamSampling, l.hasSeed, l.seed, R.transcripts, R.ti_type,
+                                hits, post, post0, R.nThreads, false);
             if (l.bamSampling) say(i, "Begin to sample reads from their posteriors.\nSampling is finished.\n");
             say(i, "Bam output file is generated!\n");
         }
@@ -220,6 +215,7 @@ int main(int argc, char* argv[]) {
             check_rc(rsem_b200_batch_slots(batch, &n_slots), "batch_slots");
             std::vector<rsem_b200_round_stats> st((size_t)n_slots * CHUNK);
             std::vector<int32_t> ran(n_slots), stopped(n_slots);
+            L.where = "the batch of its " + std::to_string(in_batch.size()) + " samples";
             {
                 Timed tk{ph.frozen};
                 check_rc(rsem_b200_batch_run(batch, CHUNK, st.data(), ran.data(), stopped.data()), "batch_run");
@@ -230,6 +226,7 @@ int main(int argc, char* argv[]) {
                 for (int r = 0; r < ran[s]; ++r) say(p.idx, round_line(p.round + 1 + r, st[(size_t)s * CHUNK + r]));
                 if (ran[s] > 0) { p.round += ran[s]; p.totNum = st[(size_t)s * CHUNK + ran[s] - 1].totnum; }
                 if (!stopped[s]) { ++it; continue; }
+                L.where = sample_at(p.idx);
                 const Line& l = lines[p.idx];
                 std::vector<double> theta(M + 1), counts(M + 1), post, post0;
                 if (l.genBam) { post.resize(p.hits.H); post0.resize(p.hits.N); }
@@ -245,7 +242,8 @@ int main(int argc, char* argv[]) {
         }
     };
 
-    for (size_t i = 0; i < lines.size(); ++i) {
+    for (size_t i; (i = claims.next()) < lines.size();) {
+        L.where = sample_at(i);
         const Line& l = lines[i];
         if (g_verbose || l.N1 == 0) block[i] += "== sample " + l.outName + " (" + manifest + " line " + std::to_string(l.no) + ")\n";
         if (l.N1 == 0) {  // EM.cpp:615-638
@@ -255,8 +253,8 @@ int main(int argc, char* argv[]) {
             fo = fopen((l.statName + ".model").c_str(), "w");
             if (fo) fclose(fo);
             std::vector<double> theta(M + 1, 0.0), eel(M + 1, 0.0), countv(M + 1, 0.0);
-            for (int t = 1; t <= M; ++t) eel[t] = transcripts[t].length;
-            write_results_em(refName, l.imdName, transcripts, theta, eel, countv.data(), l.appendNames);
+            for (int t = 1; t <= M; ++t) eel[t] = R.transcripts[t].length;
+            write_results_em(refName, l.imdName, R.transcripts, theta, eel, countv.data(), l.appendNames);
             if (l.genBam) {  // EM.cpp:627-633: the input is copied as it is
                 const std::string command = "cp " + l.inpSamF + " " + l.outName + ".transcript.bam";
                 block[i] += command + "\n";
@@ -345,18 +343,18 @@ int main(int argc, char* argv[]) {
             int rc = rsem_b200_batch_add(batch, hits.N, hits.H, M, hits.row_ptr.data(), hits.sid.data(), p->conprb.data(),
                                          p->ncpv.data(), theta.data(), (double)l.N0, ROUND + 1, MIN_ROUND, MAX_ROUND, &slot);
             if (rc == RSEM_B200_ERR_FULL) {
-                ++n_full;
+                ++L.n_full;
                 drain();
                 rc = rsem_b200_batch_add(batch, hits.N, hits.H, M, hits.row_ptr.data(), hits.sid.data(), p->conprb.data(),
                                          p->ncpv.data(), theta.data(), (double)l.N0, ROUND + 1, MIN_ROUND, MAX_ROUND, &slot);
             }
             if (rc == 0) {
-                ++n_batched;
+                ++L.n_batched;
                 in_batch[slot] = std::move(p);
                 continue;
             }
             if (rc != RSEM_B200_ERR_UNSUPPORTED && rc != RSEM_B200_ERR_FULL) check_rc(rc, "batch_add");
-            ++n_single;
+            ++L.n_single;
             std::vector<rsem_b200_round_stats> cs(32);
             Timed tk{ph.frozen};
             while (keep_going) {
@@ -381,19 +379,89 @@ int main(int argc, char* argv[]) {
         finish(i, hits, mdl, theta, counts, post, post0, p->conprb, p->ncpv, tot);
     }
     drain();
-    double k12_ms = 0;
-    uint64_t k12_rounds = 0;
-    check_rc(rsem_b200_batch_timing(batch, &k12_ms, &k12_rounds), "batch_timing");
-    if (getenv("RSEM_B200_TIMING")) {
-        fprintf(stderr, "rsem-run-em-batch timing: %d samples in the batch, %d on the single-sample path; K12 %.3f ms over %llu "
-                "sample-rounds\n", n_batched, n_single, k12_ms, (unsigned long long)k12_rounds);
-        fprintf(stderr, "rsem-run-em-batch timing: arena full %d times\n", n_full);
-        fprintf(stderr, "rsem-run-em-batch timing: load %.3f s, model rounds %.3f s, frozen rounds %.3f s, final pass %.3f s, "
-                "writers %.3f s\n", ph.load, ph.model, ph.frozen, ph.final, ph.write);
+    check_rc(rsem_b200_batch_timing(batch, &L.k12_ms, &L.k12_rounds), "batch_timing");
+}
+
+}  // namespace
+
+int main(int argc, char* argv[]) {
+    if (argc < 4) usage();
+    const time_t t_start = time(NULL);
+    Run R;
+    R.refName = argv[1];
+    R.manifest = argv[3];
+    R.read_type = atoi(argv[2]);
+    for (int i = 4; i < argc; ++i) {
+        if (!strcmp(argv[i], "-p") && i + 1 < argc) R.nThreads = atoi(argv[i + 1]);
+        if (!strcmp(argv[i], "-q")) g_verbose = false;
     }
-    rsem_b200_batch_destroy(batch);
-    rsem_b200_ctx_destroy(ctx);
-    for (const std::string& b : block) fputs(b.c_str(), stdout);
+    if (R.nThreads <= 0) die("Number of threads should be bigger than 0!");
+    g_io_threads = env_int("RSEM_B200_IO_THREADS", R.nThreads);
+    if (R.read_type < 0 || R.read_type > 3) { fprintf(stderr, "Unknown Read Type!\n"); exit(-1); }
+    R.lines = read_manifest(R.manifest, R.read_type);
+    R.MAX_ROUND = env_int("RSEM_MAX_ROUND", 10000);
+    R.MIN_ROUND = env_int("RSEM_MIN_ROUND", 20);
+
+    const std::vector<int> devices = gpu_devices();
+    std::future<LaneContexts> ctx_future = std::async(std::launch::async, open_lanes, devices);
+    load_refs(R.refName + ".seq", true, R.refs);
+    R.M = R.refs.M;
+    load_transcripts(R.refName + ".ti", R.transcripts, &R.ti_type);
+    std::vector<Lane> lanes(devices.size());
+    {
+        const LaneContexts lc = ctx_future.get();
+        if (!lc.err.empty()) die(lc.err);
+        for (size_t k = 0; k < lanes.size(); ++k) {
+            lanes[k].device = devices[k];
+            lanes[k].ctx = lc.ctx[k];
+            lanes[k].arena = lc.arena[k];
+        }
+    }
+    R.block.resize(R.lines.size());
+    Claims claims(R.lines.size());
+    if (lanes.size() == 1) {
+        run_lane(R, lanes[0], claims);
+    } else {
+        auto lane_main = [&](Lane& L) {
+            DieThrows throws(true);
+            try {
+                run_lane(R, L, claims);
+            } catch (const std::exception& e) {
+                claims.fail("rsem-run-em-batch: device " + std::to_string(L.device) + ", " + L.where + ": " + e.what());
+            }
+        };
+        std::vector<std::thread> pool;
+        for (size_t k = 1; k < lanes.size(); ++k) pool.emplace_back(lane_main, std::ref(lanes[k]));
+        lane_main(lanes[0]);
+        for (auto& th : pool) th.join();
+        if (claims.failed()) die(claims.message());
+    }
+    if (getenv("RSEM_B200_TIMING")) {
+        Lane t;   // the totals
+        for (const Lane& L : lanes) {
+            t.n_batched += L.n_batched; t.n_single += L.n_single; t.n_full += L.n_full;
+            t.k12_ms += L.k12_ms; t.k12_rounds += L.k12_rounds;
+            t.ph.load += L.ph.load; t.ph.model += L.ph.model; t.ph.frozen += L.ph.frozen; t.ph.final += L.ph.final;
+            t.ph.write += L.ph.write;
+        }
+        fprintf(stderr, "rsem-run-em-batch timing: %d samples in the batch, %d on the single-sample path; K12 %.3f ms over %llu "
+                "sample-rounds\n", t.n_batched, t.n_single, t.k12_ms, (unsigned long long)t.k12_rounds);
+        fprintf(stderr, "rsem-run-em-batch timing: arena full %d times\n", t.n_full);
+        fprintf(stderr, "rsem-run-em-batch timing: load %.3f s, model rounds %.3f s, frozen rounds %.3f s, final pass %.3f s, "
+                "writers %.3f s\n", t.ph.load, t.ph.model, t.ph.frozen, t.ph.final, t.ph.write);
+        if (lanes.size() > 1)
+            for (size_t k = 0; k < lanes.size(); ++k) {
+                const Lane& L = lanes[k];
+                fprintf(stderr, "rsem-run-em-batch timing: lane %zu, device %d: %d samples in the batch, %d on the single-sample "
+                        "path, arena full %d times; K12 %.3f ms; model rounds %.3f s, frozen rounds %.3f s, final pass %.3f s\n", k,
+                        L.device, L.n_batched, L.n_single, L.n_full, L.k12_ms, L.ph.model, L.ph.frozen, L.ph.final);
+            }
+    }
+    for (Lane& L : lanes) {
+        rsem_b200_batch_destroy(L.batch);
+        rsem_b200_ctx_destroy(L.ctx);
+    }
+    for (const std::string& b : R.block) fputs(b.c_str(), stdout);
     const time_t t_end = time(NULL);
     printf("Time Used for EM.cpp : %d h %02d m %02d s\n", int((t_end - t_start) / 3600), int((t_end - t_start) % 3600 / 60), int((t_end - t_start) % 60));
     return 0;

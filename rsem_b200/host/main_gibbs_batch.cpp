@@ -4,12 +4,20 @@
 //
 // Each non-empty manifest line is what rsem-run-gibbs takes after reference_name:
 //   imdName statName BURNIN NSAMPLES GAP [-p #chains] [--seed s] [--pseudo-count c] [--prior file]
-// and each line gets the files `rsem-run-gibbs refName <line>` writes.  One CUDA context (RSEM_B200_DEVICE) serves the whole
-// run.  A sample of 1248 .. 2^19 reads joins a Gibbs batch (K13, rsem_b200_gibbs_batch_*), which runs the chains of all its
-// samples in one launch; any other sample runs on the context with rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains, as in
-// rsem-run-gibbs.  When the batch arena is full, the samples in it are run and written before the next one is added; a
-// sample that still does not fit then runs on the context.  RSEM_B200_BATCH_ARENA_BYTES sets the arena's size
-// (default, or 0: half of the device memory free at the start).  Standard output has one block per sample, in manifest order.
+// and each line gets the files `rsem-run-gibbs refName <line>` writes.  A lane (a host thread, a CUDA context and a batch
+// arena) takes the samples one by one.  A sample of 1248 .. 2^19 reads joins the lane's Gibbs batch (K13,
+// rsem_b200_gibbs_batch_*), which runs the chains of all its samples in one launch; any other sample runs on the lane's
+// context with rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains, as in rsem-run-gibbs.  When the batch arena is full,
+// the samples in it are run and written before the next one is added; a sample that still does not fit then runs on the
+// context.
+// There is one lane on RSEM_B200_DEVICE (default 0), or one per entry of RSEM_B200_DEVICES=0,1,... when it lists more
+// than one; an entry may repeat a device (0,0 runs two lanes on device 0, whose host stages overlap).  The lanes take the
+// manifest lines in manifest order from one counter; a chain's draws depend only on its seed and its sample, so the files
+// do not depend on the lane that ran it.  Both kinds of launch are cooperative grids sized to a whole device, so the lanes
+// on one device take turns: a per-device mutex is held from before each launch until its stream has finished it.
+// RSEM_B200_BATCH_ARENA_BYTES sets each lane's arena (default, or 0: half of the device memory free at the start, shared
+// evenly by the lanes on one device).  The first failure of any lane ends the run with exit status -1 once the other lanes
+// have finished their current samples.  Standard output has one block per sample, in manifest order.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -61,8 +69,7 @@ void usage() {
 }
 
 [[noreturn]] void refuse(const std::string& manifest, int no, const std::string& why) {
-    fprintf(stderr, "%s line %d: %s\n", manifest.c_str(), no, why.c_str());
-    exit(-1);
+    die(manifest + " line " + std::to_string(no) + ": " + why);
 }
 
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
@@ -141,50 +148,65 @@ struct Phases {
     int teams = 0, workers = 0, batched = 0, single = 0, full = 0;
 };
 
-}  // namespace
-
-int main(int argc, char* argv[]) {
-    if (argc < 3) usage();
-    const std::string refName = argv[1], manifest = argv[2];
+// what every lane reads
+struct Run {
+    std::string refName, manifest;
     bool verbose = true;
-    for (int i = 3; i < argc; ++i)
-        if (!strcmp(argv[i], "-q")) verbose = false;
-    g_verbose = false;   // the messages of the shared loaders and writers go into the samples' blocks instead
-    {   // as rsem-run-gibbs: file parsing and writing use the host's cores
-        const char* e = getenv("RSEM_B200_IO_THREADS");
-        const unsigned hw = std::thread::hardware_concurrency();
-        g_io_threads = e ? atoi(e) : (int)std::min<unsigned>(hw ? hw : 1, 32);
-    }
+    int M = 0, m = 0;
+    size_t acc_per = 0;
+    bool alleleS = false;
+    std::vector<Line> lines;
     RefData refs;
-    load_refs(refName + ".seq", false, refs);
-    const int M = refs.M;
-    const std::vector<Line> lines = read_manifest(manifest, M);
-
-    struct CtxResult { int rc; rsem_b200_ctx* ctx; std::string err; };
-    std::future<CtxResult> ctx_future = std::async(std::launch::async, []() {
-        CtxResult r{0, nullptr, ""};
-        const char* d = getenv("RSEM_B200_DEVICE");
-        r.rc = rsem_b200_ctx_create(d ? atoi(d) : 0, &r.ctx);
-        if (r.rc != 0) r.err = rsem_b200_last_error();
-        return r;
-    });
     std::vector<int> gi, gt, ta;
-    load_groups(refName + ".grp", gi);
-    const int m = (int)gi.size() - 1;
-    const bool alleleS = load_allele_groups(refName, gt, ta);
-    const size_t acc_per = 4 * ((size_t)M + 1) + (size_t)m;
-
-    Phases ph;
-    std::vector<std::string> block(lines.size());
+    std::vector<std::string> block;   // standard output of each sample
     std::mutex block_mu;
+};
+
+struct Lane {
+    int device = 0;
+    rsem_b200_ctx* ctx = nullptr;
+    uint64_t arena = 0;
+    rsem_b200_gibbs_batch* batch = nullptr;
+    std::mutex* launch_mu = nullptr;   // shared by the lanes on this device
+    bool isolated = false;             // die() throws on the lane's threads (more than one lane)
+    std::string where = "no sample yet";   // what the lane is working on, for the failure message
+    Phases ph;
+    std::vector<std::pair<double, double>> launches;   // host clock around every cooperative launch, under launch_mu
+};
+
+// the samples a lane takes from `claims`, loaded, run and written on the lane's context and batch
+void run_lane(Run& R, Lane& L, Claims& claims) {
+    const std::vector<Line>& lines = R.lines;
+    const std::string& refName = R.refName;
+    const int M = R.M, m = R.m;
+    const size_t acc_per = R.acc_per;
+    const RefData& refs = R.refs;
+    const std::vector<int>& gi = R.gi;
+    const std::vector<int>& ta = R.ta;
+    const bool alleleS = R.alleleS, verbose = R.verbose;
+    rsem_b200_ctx* ctx = L.ctx;
+    Phases& ph = L.ph;
+    check_rc(rsem_b200_gibbs_batch_create(ctx, L.arena, 0, &L.batch), "gibbs_batch_create");
+    rsem_b200_gibbs_batch* batch = L.batch;
     auto say = [&](size_t i, const std::string& s) {
         if (!verbose) return;
-        std::lock_guard<std::mutex> g(block_mu);
-        block[i] += s;
+        std::lock_guard<std::mutex> g(R.block_mu);
+        R.block[i] += s;
+    };
+    auto sample_at = [&](size_t i) {
+        return "sample " + lines[i].imdName + " (" + R.manifest + " line " + std::to_string(lines[i].no) + ")";
+    };
+    // a cooperative launch: one at a time per device
+    auto launch = [&](const auto& run) {
+        std::lock_guard<std::mutex> g(*L.launch_mu);
+        const double t0 = now_s();
+        run();
+        L.launches.emplace_back(t0, now_s());
     };
 
     // a sample's inputs (rsem-run-gibbs's load_data, load_omit_info / load_prior_info, init_model_related, init)
     auto load = [&](size_t i) {
+        DieThrows throws(L.isolated);
         const Line& l = lines[i];
         auto s = std::make_unique<Sample>();
         s->idx = i;
@@ -237,16 +259,6 @@ int main(int argc, char* argv[]) {
         say(s.idx, "Gibbs based expression values are written!\n");
     };
 
-    rsem_b200_ctx* ctx = nullptr;
-    {
-        CtxResult r = ctx_future.get();
-        if (r.rc != 0) die("rsem_b200: ctx_create failed: " + r.err);
-        ctx = r.ctx;
-    }
-    rsem_b200_gibbs_batch* batch = nullptr;
-    const char* arena = getenv("RSEM_B200_BATCH_ARENA_BYTES");
-    check_rc(rsem_b200_gibbs_batch_create(ctx, arena ? strtoull(arena, nullptr, 10) : 0, 0, &batch), "gibbs_batch_create");
-
     // the samples in the batch run in one launch; their outputs are copied back one by one and written on worker threads
     std::map<int32_t, std::unique_ptr<Sample>> in_batch;
     const int n_writers = std::max(1, std::min(g_io_threads, 8));
@@ -254,8 +266,9 @@ int main(int argc, char* argv[]) {
         if (in_batch.empty()) return;
         rsem_b200_gibbs_batch_stats st;
         {
+            L.where = "the batch of its " + std::to_string(in_batch.size()) + " samples";
             const double t0 = now_s();
-            check_rc(rsem_b200_gibbs_batch_run(batch, &st), "gibbs_batch_run");
+            launch([&]() { check_rc(rsem_b200_gibbs_batch_run(batch, &st), "gibbs_batch_run"); });
             ph.device += now_s() - t0;
         }
         ph.k13_ms += st.device_ms;
@@ -269,8 +282,10 @@ int main(int argc, char* argv[]) {
         std::atomic<size_t> next{0};
         std::mutex copy_mu;
         std::vector<double> t_copy(n_writers, 0.0), t_write(n_writers, 0.0);
+        std::exception_ptr failed;   // a writer's first failure, raised on the lane's thread once every writer has stopped
         auto writer = [&](int w) {
-            for (size_t k; (k = next.fetch_add(1)) < todo.size();) {
+            DieThrows throws(L.isolated);
+            for (size_t k; (k = next.fetch_add(1)) < todo.size();) try {
                 const Sample& s = *todo[k].second;
                 std::vector<int32_t> cvs((size_t)lines[s.idx].nsamples * (M + 1));
                 std::vector<double> acc(s.chain_samples.size() * acc_per);
@@ -283,6 +298,10 @@ int main(int argc, char* argv[]) {
                 const double t1 = now_s();
                 finish(s, cvs, acc);
                 t_write[w] += now_s() - t1;
+            } catch (...) {
+                std::lock_guard<std::mutex> g(copy_mu);
+                if (!failed) { failed = std::current_exception(); L.where = sample_at(todo[k].second->idx); }
+                next = todo.size();
             }
         };
         {
@@ -291,27 +310,29 @@ int main(int argc, char* argv[]) {
             writer(0);
             for (auto& th : pool) th.join();
         }
+        if (failed) std::rethrow_exception(failed);
         for (int w = 0; w < n_writers; ++w) { ph.copy += t_copy[w]; ph.write += t_write[w]; }
         check_rc(rsem_b200_gibbs_batch_clear(batch), "gibbs_batch_clear");
         in_batch.clear();
     };
 
-    // loading runs a few samples ahead of the adds, on host threads
-    const size_t ahead = 4;
-    std::deque<std::future<std::unique_ptr<Sample>>> loads;
-    size_t next_load = 0;
+    // loading runs a few samples ahead of the adds, on host threads; with several lanes, whose loads overlap anyway, one
+    // line ahead, so that a lane holds few lines the others could take
+    const size_t ahead = L.isolated ? 2 : 4;
+    std::deque<std::pair<size_t, std::future<std::unique_ptr<Sample>>>> loads;
     auto top_up = [&]() {
-        while (next_load < lines.size() && loads.size() < ahead) {
-            const size_t i = next_load++;
-            loads.push_back(std::async(std::launch::async, load, i));
+        while (loads.size() < ahead) {
+            const size_t i = claims.next();
+            if (i >= lines.size()) break;
+            loads.emplace_back(i, std::async(std::launch::async, load, i));
         }
     };
-    for (size_t i = 0; i < lines.size(); ++i) {
+    for (top_up(); !loads.empty(); top_up()) {
+        const size_t i = loads.front().first;
+        L.where = sample_at(i);
         const Line& l = lines[i];
-        if (verbose) block[i] += "== sample " + l.imdName + " (" + manifest + " line " + std::to_string(l.no) + ")\n";
-        top_up();
         const double t_load = now_s();
-        std::unique_ptr<Sample> s = loads.front().get();
+        std::unique_ptr<Sample> s = loads.front().second.get();
         loads.pop_front();
         say(i, "Refs.loadRefs finished!\nLoading data is finished!\nLoading group information is finished!\nGibbs started!\nInitialization finished!\n");
         const rsem_b200_gibbs_params gp = params_of(*s);
@@ -342,16 +363,86 @@ int main(int argc, char* argv[]) {
         std::vector<int32_t> cvs((size_t)l.nsamples * (M + 1));
         std::vector<double> acc(s->chain_samples.size() * acc_per);
         rsem_b200_gibbs_stats gs;
-        check_rc(rsem_b200_gibbs_run_chains(ctx, &gp, cvs.data(), acc.data(), &gs), "gibbs_run");
+        launch([&]() { check_rc(rsem_b200_gibbs_run_chains(ctx, &gp, cvs.data(), acc.data(), &gs), "gibbs_run"); });
         const double t1 = now_s();
         ph.device += t1 - t0;
         finish(*s, cvs, acc);
         ph.write += now_s() - t1;
     }
     drain();
+}
+
+}  // namespace
+
+int main(int argc, char* argv[]) {
+    if (argc < 3) usage();
+    Run R;
+    R.refName = argv[1];
+    R.manifest = argv[2];
+    for (int i = 3; i < argc; ++i)
+        if (!strcmp(argv[i], "-q")) R.verbose = false;
+    g_verbose = false;   // the messages of the shared loaders and writers go into the samples' blocks instead
+    {   // as rsem-run-gibbs: file parsing and writing use the host's cores
+        const char* e = getenv("RSEM_B200_IO_THREADS");
+        const unsigned hw = std::thread::hardware_concurrency();
+        g_io_threads = e ? atoi(e) : (int)std::min<unsigned>(hw ? hw : 1, 32);
+    }
+    load_refs(R.refName + ".seq", false, R.refs);
+    R.M = R.refs.M;
+    R.lines = read_manifest(R.manifest, R.M);
+
+    const std::vector<int> devices = gpu_devices();
+    std::future<LaneContexts> ctx_future = std::async(std::launch::async, open_lanes, devices);
+    load_groups(R.refName + ".grp", R.gi);
+    R.m = (int)R.gi.size() - 1;
+    R.alleleS = load_allele_groups(R.refName, R.gt, R.ta);
+    R.acc_per = 4 * ((size_t)R.M + 1) + (size_t)R.m;
+    R.block.resize(R.lines.size());
+    if (R.verbose)
+        for (size_t i = 0; i < R.lines.size(); ++i)
+            R.block[i] = "== sample " + R.lines[i].imdName + " (" + R.manifest + " line " + std::to_string(R.lines[i].no) + ")\n";
+
+    std::vector<Lane> lanes(devices.size());
+    std::map<int, std::mutex> launch_mu;
+    {
+        const LaneContexts lc = ctx_future.get();
+        if (!lc.err.empty()) die(lc.err);
+        for (size_t k = 0; k < lanes.size(); ++k) {
+            lanes[k].device = devices[k];
+            lanes[k].ctx = lc.ctx[k];
+            lanes[k].arena = lc.arena[k];
+            lanes[k].launch_mu = &launch_mu[devices[k]];
+            lanes[k].isolated = lanes.size() > 1;
+        }
+    }
+    Claims claims(R.lines.size());
+    if (lanes.size() == 1) {
+        run_lane(R, lanes[0], claims);
+    } else {
+        auto lane_main = [&](Lane& L) {
+            DieThrows throws(true);
+            try {
+                run_lane(R, L, claims);
+            } catch (const std::exception& e) {
+                claims.fail("rsem-run-gibbs-batch: device " + std::to_string(L.device) + ", " + L.where + ": " + e.what());
+            }
+        };
+        std::vector<std::thread> pool;
+        for (size_t k = 1; k < lanes.size(); ++k) pool.emplace_back(lane_main, std::ref(lanes[k]));
+        lane_main(lanes[0]);
+        for (auto& th : pool) th.join();
+        if (claims.failed()) die(claims.message());
+    }
     if (getenv("RSEM_B200_TIMING")) {
+        Phases ph;   // the totals
+        for (const Lane& L : lanes) {
+            ph.load += L.ph.load; ph.device += L.ph.device; ph.copy += L.ph.copy; ph.write += L.ph.write;
+            ph.k13_ms += L.ph.k13_ms; ph.chain_cycles += L.ph.chain_cycles; ph.sample_cycles += L.ph.sample_cycles;
+            ph.jobs += L.ph.jobs; ph.batched += L.ph.batched; ph.single += L.ph.single; ph.full += L.ph.full;
+            if (L.ph.teams) { ph.teams = L.ph.teams; ph.workers = L.ph.workers; }
+        }
         uint64_t cv_bytes = 0;
-        for (const Line& l : lines)
+        for (const Line& l : R.lines)
             for (int t = 0; t < l.nThreads; ++t) {
                 FILE* f = fopen((l.imdName + ".countvectors" + std::to_string(t)).c_str(), "rb");
                 if (!f) continue;
@@ -366,9 +457,24 @@ int main(int argc, char* argv[]) {
         fprintf(stderr, "rsem-run-gibbs-batch timing: load+components %.3f s, device %.3f s, copies back %.3f s, writers %.3f s "
                 "(thread seconds), count-vector text %llu bytes\n", ph.load, ph.device, ph.copy, ph.write, (unsigned long long)cv_bytes);
         fprintf(stderr, "rsem-run-gibbs-batch timing: arena full %d times\n", ph.full);
+        if (lanes.size() > 1)
+            for (size_t k = 0; k < lanes.size(); ++k) {   // launches: start-end of each, host monotonic clock in seconds
+                const Lane& L = lanes[k];
+                std::string stamps;
+                char buf[64];
+                for (const auto& t : L.launches) {
+                    snprintf(buf, sizeof buf, " %.6f-%.6f", t.first, t.second);
+                    stamps += buf;
+                }
+                fprintf(stderr, "rsem-run-gibbs-batch timing: lane %zu, device %d: %d samples in the batch, %d on the single-sample "
+                        "path, arena full %d times; device %.3f s; launches%s\n", k, L.device, L.ph.batched, L.ph.single, L.ph.full,
+                        L.ph.device, stamps.c_str());
+            }
     }
-    rsem_b200_gibbs_batch_destroy(batch);
-    rsem_b200_ctx_destroy(ctx);
-    for (const std::string& b : block) fputs(b.c_str(), stdout);
+    for (Lane& L : lanes) {
+        rsem_b200_gibbs_batch_destroy(L.batch);
+        rsem_b200_ctx_destroy(L.ctx);
+    }
+    for (const std::string& b : R.block) fputs(b.c_str(), stdout);
     return 0;
 }

@@ -30,7 +30,7 @@ void LenDistH::zero() {
 void LenDistH::finish() {  // LenDist.h:186-200
     double sum = 0.0;
     for (int i = 1; i <= span; ++i) sum += pdf[i];
-    if (sum <= kEps) { fprintf(stderr, "No valid read to estimate the length distribution!\n"); exit(-1); }
+    if (sum <= kEps) die("No valid read to estimate the length distribution!");
     for (int i = 1; i <= span; ++i) {
         pdf[i] = pdf[i] / sum;
         cdf[i] = cdf[i - 1] + pdf[i];
@@ -63,8 +63,8 @@ void LenDistH::set_as_normal(double mean, double sd, int minL, int maxL) {  // L
     const int meanL = int(mean + .5);
     if (sd < kEps) {
         if (meanL < minL || meanL > maxL) {
-            fprintf(stderr, "Length distribution's probability mass is not within the possible range! MeanL = %d, MinL = %d, MaxL = %d\n", meanL, minL, maxL);
-            exit(-1);
+            die("Length distribution's probability mass is not within the possible range! MeanL = " + std::to_string(meanL) +
+                ", MinL = " + std::to_string(minL) + ", MaxL = " + std::to_string(maxL));
         }
         span = 1;
         lb = meanL - 1;

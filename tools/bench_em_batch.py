@@ -8,9 +8,12 @@ Every run is free-running (no RSEM_MAX_ROUND).  --reference times the reference 
 Prints one JSON line per workload: wall time per sample of each program, K12 device time per sample-round (CUDA
 events), K12's achieved bytes/s on 12 H + 16 N + 16 (m + 1) per sample-round against 3.35 TB/s, the phase split of
 the batch run, and the card's name and power limit read in the same run.
+With --devices LIST (e.g. 0,0 or 0,1,2,3) it times rsem-run-em-batch alone instead: --repeats times on one device and
+with RSEM_B200_DEVICES=LIST, alternating, on two copies of the samples whose .theta must agree to 1e-6 relative, and
+prints the best wall time per sample of each.
 
   python tools/bench_em_batch.py [--samples 264] [--reads-min 50000] [--reads-max 500000] [--bulk-samples 3]
-                                 [--bulk-reads 2000000] [--reference] [--workdir DIR]
+                                 [--bulk-reads 2000000] [--reference] [--devices LIST [--repeats 2]] [--workdir DIR]
 """
 import argparse
 import json
@@ -65,12 +68,15 @@ def frozen_bytes_per_round(d):
     return 12 * len(sid) + 16 * (len(row_ptr) - 1) + 16 * (len(np.unique(np.abs(sid))) + 1)
 
 
-def run_batch(root, dirs):
+def run_batch(root, dirs, devices=None):
     with open(os.path.join(root, "manifest"), "w") as f:
         for d in dirs:
             b = os.path.basename(d)
             f.write(f"{b}/s {b}/s.temp/s {b}/s.stat/s\n")
     env = dict(os.environ, RSEM_B200_TIMING="1")
+    env.pop("RSEM_B200_DEVICES", None)
+    if devices:
+        env["RSEM_B200_DEVICES"] = devices
     t0 = time.perf_counter()
     p = subprocess.run([os.path.join(rf.BIN_DIR, "rsem-run-em-batch"), f"{os.path.basename(dirs[0])}/ref/r", "0",
                         "manifest", "-p", str(os.cpu_count())], cwd=root, env=env, stdout=subprocess.PIPE,
@@ -134,6 +140,21 @@ def workload(name, root, dirs, reference):
     return out
 
 
+def devices_workload(name, root, dirs, devices, repeats):
+    """rsem-run-em-batch on one device and on `devices`, alternating, each in its own copy of the samples"""
+    lanes_root = root + ".lanes"
+    shutil.copytree(root, lanes_root, symlinks=True)
+    lanes_dirs = [os.path.join(lanes_root, os.path.basename(d)) for d in dirs]
+    one, lanes = [], []
+    for r in range(repeats):
+        one.append(run_batch(root, dirs)[0])
+        lanes.append(run_batch(lanes_root, lanes_dirs, devices)[0])
+        log(f"{name}: repeat {r}: one device {one[-1]:.2f} s, RSEM_B200_DEVICES={devices} {lanes[-1]:.2f} s")
+    check_same(dirs, lanes_dirs, f"RSEM_B200_DEVICES={devices}")
+    return dict(workload=name, samples=len(dirs), devices=devices, repeats=repeats,
+                one_device_s_per_sample=min(one) / len(dirs), devices_s_per_sample=min(lanes) / len(dirs))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--samples", type=int, default=264)
@@ -144,6 +165,8 @@ def main():
     ap.add_argument("--bulk-samples", type=int, default=3)
     ap.add_argument("--bulk-reads", type=int, default=2000000)
     ap.add_argument("--reference", action="store_true")
+    ap.add_argument("--devices", default=None, help="RSEM_B200_DEVICES list to time against one device")
+    ap.add_argument("--repeats", type=int, default=2)
     ap.add_argument("--workdir", default=None)
     a = ap.parse_args()
     name, power = card()
@@ -156,7 +179,10 @@ def main():
             root = os.path.join(work, wl)
             os.makedirs(root, exist_ok=True)
             dirs = generate(root, n, lo, hi, a.M, frac, seed=len(wl))
-            res = workload(wl, root, dirs, a.reference and wl == "single-cell")
+            if a.devices:
+                res = devices_workload(wl, root, dirs, a.devices, a.repeats)
+            else:
+                res = workload(wl, root, dirs, a.reference and wl == "single-cell")
             res.update(M=a.M, reads=[lo, hi], expressed_frac=frac, gpu=name, power_limit=power)
             print(json.dumps(res), flush=True)
     finally:

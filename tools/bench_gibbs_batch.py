@@ -13,9 +13,13 @@ compared with bin/rsem-run-gibbs's before any time is printed.  Prints one JSON 
 both programs (and of the reference), K13 device time (CUDA events), the share of chain cycles spent in the per-kept-draw
 O(M) work (ChainSync::prof[3]), the phase split of the batch run, the bytes of count-vector text written, and the card's
 name and power limit read in the same run.  The work directory is deleted at the end.
+With --devices LIST (e.g. 0,0 or 0,1,2,3) it times rsem-run-gibbs-batch alone instead: --repeats times on one device and
+with RSEM_B200_DEVICES=LIST, alternating, on two copies of the samples whose output files must be byte-identical, and
+prints the best wall time per sample of each.
 
   python tools/bench_gibbs_batch.py [--samples 16] [--reads 75000] [--bulk-samples 1] [--bulk-reads 600000]
-                                    [--transcripts 50000] [--reference] [--reference-seconds 600] [--workdir DIR]
+                                    [--transcripts 50000] [--reference] [--reference-seconds 600]
+                                    [--devices LIST [--repeats 2]] [--workdir DIR]
 """
 import argparse
 import filecmp
@@ -63,6 +67,42 @@ def files(k):
     return [f"d{k}/s.temp/s.countvectors{t}" for t in range(THREADS)] + [f"d{k}/s.temp/s.iso_res", f"d{k}/s.temp/s.gene_res"]
 
 
+def run_batch(root, devices=None):
+    env = dict(os.environ, RSEM_B200_TIMING="1")
+    env.pop("RSEM_B200_DEVICES", None)
+    if devices:
+        env["RSEM_B200_DEVICES"] = devices
+    t0 = time.time()
+    p = subprocess.run([os.path.join(rf.BIN_DIR, "rsem-run-gibbs-batch"), "d0/ref/r", "manifest", "-q"], cwd=root, env=env,
+                       capture_output=True, text=True)
+    if p.returncode != 0:
+        raise RuntimeError(p.stderr[-3000:])
+    return time.time() - t0, p
+
+
+def devices_workload(work, name, n, reads, M, spurious, frac, devices, repeats):
+    """rsem-run-gibbs-batch on one device and on `devices`, alternating, each in its own copy of the samples"""
+    root = os.path.join(work, name)
+    log(f"{name}: generating {n} samples of {reads} reads")
+    make(root, n, reads, M, spurious, frac)
+    with open(os.path.join(root, "manifest"), "w") as f:
+        f.write("".join(f"d{k}/s.temp/s d{k}/s.stat/s {GIBBS_ARGS} --seed {17 + k}\n" for k in range(n)))
+    lanes = root + ".lanes"
+    shutil.copytree(root, lanes)
+    t_one, t_lanes = [], []
+    for r in range(repeats):
+        t_one.append(run_batch(root)[0])
+        t_lanes.append(run_batch(lanes, devices)[0])
+        log(f"{name}: repeat {r}: one device {t_one[-1]:.2f} s, RSEM_B200_DEVICES={devices} {t_lanes[-1]:.2f} s")
+    for k in range(n):
+        for f in files(k):
+            if not filecmp.cmp(os.path.join(root, f), os.path.join(lanes, f), shallow=False):
+                raise RuntimeError(f"{name}: {f} differs between one device and RSEM_B200_DEVICES={devices}")
+    return dict(workload=name, samples=n, reads=reads, transcripts=M, spurious=spurious, expressed_frac=frac,
+                gibbs_args=GIBBS_ARGS, devices=devices, repeats=repeats, one_device_s_per_sample=min(t_one) / n,
+                devices_s_per_sample=min(t_lanes) / n)
+
+
 def workload(work, name, n, reads, M, spurious, frac, reference, ref_seconds):
     root = os.path.join(work, name)
     log(f"{name}: generating {n} samples of {reads} reads")
@@ -72,12 +112,7 @@ def workload(work, name, n, reads, M, spurious, frac, reference, ref_seconds):
     with open(os.path.join(root, "manifest"), "w") as f:
         f.write("".join(f"d{k}/s.temp/s d{k}/s.stat/s {GIBBS_ARGS} --seed {17 + k}\n" for k in range(n)))
     log(f"{name}: rsem-run-gibbs-batch")
-    t0 = time.time()
-    p = subprocess.run([os.path.join(rf.BIN_DIR, "rsem-run-gibbs-batch"), "d0/ref/r", "manifest", "-q"], cwd=root,
-                       env=dict(os.environ, RSEM_B200_TIMING="1"), capture_output=True, text=True)
-    t_batch = time.time() - t0
-    if p.returncode != 0:
-        raise RuntimeError(p.stderr[-3000:])
+    t_batch, p = run_batch(root)
     log(f"{name}: bin/rsem-run-gibbs once per sample")
     t0 = time.time()
     for k in range(n):
@@ -127,6 +162,8 @@ def main():
     ap.add_argument("--reference-seconds", type=float, default=600.0)
     ap.add_argument("--workdir", default=None)
     ap.add_argument("--only", default=None, help="comma-separated workload names")
+    ap.add_argument("--devices", default=None, help="RSEM_B200_DEVICES list to time against one device")
+    ap.add_argument("--repeats", type=int, default=2)
     a = ap.parse_args()
     work = tempfile.mkdtemp(prefix="bench_gibbs_batch_", dir=a.workdir)
     try:
@@ -136,7 +173,10 @@ def main():
         for wl, n, reads, spurious, frac in specs:
             if a.only and wl not in a.only.split(","):
                 continue
-            res = workload(work, wl, n, reads, a.transcripts, spurious, frac, a.reference, a.reference_seconds)
+            if a.devices:
+                res = devices_workload(work, wl, n, reads, a.transcripts, spurious, frac, a.devices, a.repeats)
+            else:
+                res = workload(work, wl, n, reads, a.transcripts, spurious, frac, a.reference, a.reference_seconds)
             res.update(gpu=name, power_limit=power)
             print(json.dumps(res), flush=True)
     finally:
