@@ -3,6 +3,7 @@
 #include <sys/stat.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -83,86 +84,11 @@ uint32_t parse_seed(const char* s) {
     return seed;
 }
 
-std::vector<int> gpu_devices() {
-    std::vector<int> devices;
-    if (const char* e = getenv("RSEM_B200_DEVICES")) {  // e.g. "0,1,2,3"
-        for (const char* q = e; *q;) {
-            devices.push_back(atoi(q));
-            while (*q && *q != ',') ++q;
-            if (*q == ',') ++q;
-        }
-    }
-    if (devices.size() <= 1) {
-        const char* one = getenv("RSEM_B200_DEVICE");
-        devices.assign(1, one ? atoi(one) : devices.empty() ? 0 : devices[0]);
-    }
-    return devices;
-}
+double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-LaneContexts open_lanes(const std::vector<int>& devices) {
-    const size_t n = devices.size();
-    LaneContexts out;
-    out.ctx.assign(n, nullptr);
-    out.arena.assign(n, 0);
-    const char* e = getenv("RSEM_B200_BATCH_ARENA_BYTES");
-    const uint64_t set = e ? strtoull(e, nullptr, 10) : 0;   // 0 is the default, as unset
-    out.arena.assign(n, set);
-    const bool share = n > 1 && set == 0;
-    std::vector<std::string> err(n);
-    std::vector<int> distinct;
-    for (int d : devices)
-        if (std::find(distinct.begin(), distinct.end(), d) == distinct.end()) distinct.push_back(d);
-    // per device: its free memory, then the contexts of its lanes; the devices side by side
-    auto open_device = [&](int d) {
-        std::vector<size_t> mine;
-        for (size_t k = 0; k < n; ++k)
-            if (devices[k] == d) mine.push_back(k);
-        const std::string where = n > 1 ? "device " + std::to_string(d) + ": " : "";
-        if (share) {
-            uint64_t free_b = 0;
-            if (rsem_b200_device_free_bytes(d, &free_b) != 0) {
-                err[mine[0]] = "rsem_b200: " + where + "device_free_bytes failed: " + rsem_b200_last_error();
-                return;
-            }
-            for (size_t k : mine) out.arena[k] = free_b / 2 / mine.size();
-        }
-        for (size_t k : mine)
-            if (rsem_b200_ctx_create(d, &out.ctx[k]) != 0) {
-                err[k] = "rsem_b200: " + where + "ctx_create failed: " + rsem_b200_last_error();
-                return;
-            }
-    };
-    {
-        std::vector<std::thread> pool;
-        for (size_t j = 1; j < distinct.size(); ++j) pool.emplace_back(open_device, distinct[j]);
-        open_device(distinct[0]);
-        for (auto& th : pool) th.join();
-    }
-    for (const std::string& m : err)
-        if (!m.empty()) {
-            out.err = m;
-            break;
-        }
-    return out;
-}
-
-size_t Claims::next() {
-    if (failed_) return n_;
-    return std::min(n_, i_.fetch_add(1));
-}
-
-void Claims::fail(const std::string& msg) {
-    std::lock_guard<std::mutex> g(mu_);
-    if (failed_) return;
-    msg_ = msg;
-    failed_ = true;
-}
-
-bool Claims::failed() { return failed_; }
-
-std::string Claims::message() {
-    std::lock_guard<std::mutex> g(mu_);
-    return msg_;
+int env_int(const char* name, int dflt) {
+    const char* v = getenv(name);
+    return v ? atoi(v) : dflt;
 }
 
 namespace {

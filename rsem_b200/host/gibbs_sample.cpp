@@ -2,6 +2,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <ctime>
 
 #include "host.hpp"
 
@@ -56,6 +57,81 @@ std::string gibbs_inputs(const std::string& imdName, int M, uint64_t N0, uint64_
     return "";
 }
 
+std::string parse_gibbs_args(const std::vector<std::string>& f, GibbsArgs& a) {
+    a.imdName = f[0];
+    a.statName = f[1];
+    a.burnin = atoi(f[2].c_str());
+    a.nsamples = atoi(f[3].c_str());
+    a.gap = atoi(f[4].c_str());
+    for (size_t i = 5; i < f.size(); ++i) {
+        const bool arg = i + 1 < f.size();
+        if (f[i] == "-p" && arg) a.nThreads = atoi(f[i + 1].c_str());
+        if (f[i] == "--seed" && arg) { a.hasSeed = true; a.seed = parse_seed(f[i + 1].c_str()); }
+        if (f[i] == "--pseudo-count" && arg) a.pseudoC = atof(f[i + 1].c_str());
+        if (f[i] == "-q") a.quiet = true;
+        if (f[i] == "--prior" && arg) { a.hasPrior = true; a.fprior = f[i + 1]; }
+    }
+    if (!(a.nsamples > 1)) return "NSAMPLES must be larger than 1, otherwise the posterior variance cannot be calculated!";
+    if (a.gap < 1) return "GAP must be at least 1!";
+    return "";
+}
+
+void clamp_gibbs_chains(GibbsArgs& a) {
+    if (a.nThreads > a.nsamples) {
+        a.nThreads = a.nsamples;
+        fprintf(stderr, "Warning: Number of samples is less than number of threads! Change the number of threads to %d!\n", a.nThreads);
+    }
+    if (a.nThreads < 1) a.nThreads = 1;
+}
+
+void load_gibbs_ofg(const GibbsArgs& a, int M, GibbsSample& s, const Say& say) {
+    load_ofg(a.imdName + ".ofg", M, s.N0, s.row_ptr, s.sid, s.conprb);
+    s.N1 = s.row_ptr.size() - 1;
+    say("Loading data is finished!\n");
+}
+
+void load_gibbs_inputs(const GibbsArgs& a, const RefData& refs, GibbsSample& s, const Say& say) {
+    const int M = refs.M;
+    const std::string why = gibbs_inputs(a.imdName, M, s.N0, s.N1, a.pseudoC, a.hasPrior ? &a.fprior : nullptr, s.init_counts,
+                                         s.alpha, s.totc);
+    if (!why.empty()) die(why);
+    // init_model_related: eel from the .model's gld, mw copy
+    int model_type = 0;
+    LenDistH gld;
+    HostModel::read_for_gibbs(a.statName + ".model", M, model_type, gld, s.mw);
+    calc_eel(refs, gld, s.eel);
+    say("Gibbs started!\n");
+    // init(): samples per chain and per-chain engines (Gibbs.cpp:207-254)
+    s.chain_seeds = engine_seeds(a.hasSeed ? a.seed : (uint32_t)time(NULL), a.nThreads);
+    s.chain_samples.resize(a.nThreads);
+    const int quotient = a.nsamples / a.nThreads, left = a.nsamples % a.nThreads;
+    for (int t = 0; t < a.nThreads; ++t) s.chain_samples[t] = quotient + (t < left ? 1 : 0);
+    say("Initialization finished!\n");
+}
+
+rsem_b200_gibbs_params gibbs_params(const GibbsArgs& a, const GibbsSample& s, const std::vector<int>& gi) {
+    rsem_b200_gibbs_params gp;
+    memset(&gp, 0, sizeof gp);
+    gp.M = (int)s.init_counts.size() - 1;
+    gp.burnin = a.burnin;
+    gp.gap = a.gap;
+    gp.n_chains = (int)s.chain_samples.size();
+    gp.chain_samples = s.chain_samples.data();
+    gp.chain_seeds = s.chain_seeds.data();
+    gp.n0 = (double)s.N0;
+    gp.init_counts = s.init_counts.data();
+    gp.pseudo_counts = s.alpha.data();
+    gp.totc = s.totc;
+    gp.eel = s.eel.data();
+    gp.mw = s.mw.data();
+    gp.n_genes = (int)gi.size() - 1;
+    gp.gene_start = gi.data();
+    return gp;
+}
+
+namespace {
+
+// imdName.countvectors<t>, one per chain (Gibbs.cpp:257-262); cvs holds the chains' vectors in chain order
 void write_countvectors(const std::string& imdName, int M, const std::vector<int32_t>& chain_samples, const int32_t* cvs) {
     size_t at = 0;
     std::vector<char> buf(1 << 20);
@@ -72,6 +148,8 @@ void write_countvectors(const std::string& imdName, int M, const std::vector<int
     }
 }
 
+// release() (Gibbs.cpp:399-422): means and unbiased variances from the sums of all chains and the kept count vectors,
+// then imdName.iso_res / gene_res (and the allele file) by write_results_gibbs
 void write_gibbs_results(const std::string& refName, const std::string& imdName, int M, int NSAMPLES, const std::vector<int>& gi,
                          bool alleleS, const std::vector<int>& ta, const int32_t* cvs, const std::vector<double>& sum_c,
                          const std::vector<double>& sum_c2, const std::vector<double>& sum_tpm, const std::vector<double>& sum_fpkm,
@@ -110,6 +188,23 @@ void write_gibbs_results(const std::string& refName, const std::string& imdName,
         }
     }
     write_results_gibbs(refName, imdName, M, pme_c, pme_fpkm, pme_tpm, pve_c, pve_g, pve_t);
+}
+
+}  // namespace
+
+void finish_gibbs_sample(const std::string& refName, const GibbsArgs& a, const GibbsSample& s, const std::vector<int>& gi,
+                         bool alleleS, const std::vector<int>& ta, const int32_t* cvs, const double* chain_acc, const Say& say) {
+    const int M = (int)s.init_counts.size() - 1, m = (int)gi.size() - 1;
+    std::vector<double> sum_c(M + 1), sum_c2(M + 1), sum_tpm(M + 1), sum_fpkm(M + 1), sum_g2(m);
+    rsem_b200_gibbs_out go;
+    go.count_vectors = nullptr;   // not touched by the sums
+    go.sum_c = sum_c.data(); go.sum_c2 = sum_c2.data(); go.sum_tpm = sum_tpm.data(); go.sum_fpkm = sum_fpkm.data();
+    go.sum_gene_c2 = sum_g2.data();
+    const rsem_b200_gibbs_params gp = gibbs_params(a, s, gi);
+    check_rc(rsem_b200_gibbs_sum_chains(&gp, chain_acc, &go), "gibbs_sum_chains");
+    write_countvectors(a.imdName, M, s.chain_samples, cvs);
+    say("Gibbs finished!\n");
+    write_gibbs_results(refName, a.imdName, M, a.nsamples, gi, alleleS, ta, cvs, sum_c, sum_c2, sum_tpm, sum_fpkm, sum_g2);
 }
 
 }  // namespace host

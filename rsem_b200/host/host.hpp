@@ -10,10 +10,12 @@
 #include <atomic>
 #include <cstdint>
 #include <cstdio>
+#include <ctime>
 #include <functional>
 #include <map>
 #include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "rsem_b200.h"
@@ -187,23 +189,100 @@ void expression_values(const std::vector<double>& theta, const std::vector<doubl
 void write_results_em(const std::string& ref_name, const std::string& imd_name, const std::vector<TranscriptInfo>& tr,
                       const std::vector<double>& theta, const std::vector<double>& eel, const double* counts,
                       bool append_names);  // WriteResults.h:125-355
-// em_sample.cpp: the per-sample output stages of rsem-run-em (also used by rsem-run-em-batch)
+// Where a per-sample stage sends its progress lines: stdout for the single-sample tools, the sample's block in the batch tools
+using Say = std::function<void(const std::string&)>;
+
+// ---- em_sample.cpp: the per-sample stages of rsem-run-em, which rsem-run-em-batch runs for each manifest line ----------
+struct EmReference {   // refName.seq (with the sequences) and refName.ti
+    std::string name;
+    RefData refs;
+    std::vector<TranscriptInfo> transcripts;
+    int ti_type = 0;
+};
+void load_em_reference(const std::string& refName, EmReference& ref);
+// rsem-run-em's arguments from sampleName on: sampleName imdName statName [options] (EM.cpp:578-600); -p and -q are only
+// recorded here, rsem-run-em-batch ignores them on a manifest line
+struct EmArgs {
+    std::string outName, imdName, statName, inpSamF;
+    bool genBam = false, bamSampling = false, gibbsOut = false, hasSeed = false, appendNames = false, quiet = false;
+    uint32_t seed = 0;
+    int nThreads = 1;
+};
+EmArgs parse_em_args(const std::vector<std::string>& f);   // f.size() >= 3
+struct EmCounts { uint64_t N0 = 0, N1 = 0, N2 = 0, N_tot = 0; };
+bool load_cnt(const std::string& statName, bool must_exist, EmCounts& n);   // statName.cnt; false: cannot be parsed
+// N1 == 0 (EM.cpp:615-638): empty .theta / .model, zero result rows, with -b the input copied as it is; `say` gets the
+// warning and the cp command
+void write_no_alignable_reads(const EmReference& ref, const EmArgs& a, const Say& say);
+// a sample from its counts to its outputs
+struct EmSample {
+    EmCounts n;
+    ModelParamsH mp;
+    Sidecar sidecar;             // imdName.b200 while it describes this sample, until the model is estimated
+    bool have_sidecar = false;
+    HitStore hits;
+    HostModel model;
+    std::vector<double> theta;   // the initial θ (EM.cpp:342-346), then the final one
+    std::vector<double> counts, conprb, ncpv, post, post0;   // expected counts without N0, .ofg inputs, -b posteriors
+};
+// imdName.mparams and the hits: from the side-car when it describes this sample, else from imdName.dat
+void load_em_hits(const std::string& imdName, int read_type, int M, EmSample& s);
+// then the initial θ, the master model and estimateFromReads (EM.cpp:97-174, 342-346); the alignable reads go to `reads`
+void load_em_model(const std::string& imdName, int read_type, const RefData& refs, EmSample& s, ReadStore& reads, const Say& say);
+using OnRound = std::function<void(int round, const rsem_b200_round_stats&)>;
+std::string round_line(int round, const rsem_b200_round_stats& s);   // "ROUND = ..." as EM.cpp:415 prints it
+struct EmRounds {
+    int round = 0;          // the last round run
+    long long totNum = 0;
+    bool keep_going = true;
+};
+// rounds 1-10, which update the model (EM.cpp:364-416), on ctx; they end with the model pushed and conprb computed
+EmRounds em_model_rounds(rsem_b200_ctx* ctx, HostModel& model, uint64_t N0, int MIN_ROUND, int MAX_ROUND, const OnRound& on_round);
+// the frozen rounds that follow on ctx, 32 per rsem_b200_em_rounds call, until the stop rule holds
+void em_frozen_rounds(rsem_b200_ctx* ctx, uint64_t N0, int MIN_ROUND, int MAX_ROUND, EmRounds& r, const OnRound& on_round);
+// the end of a sample whose EM has ended: the convergence warning (prefixed with `who`), .ofg with --gibbs-out,
+// counts[0] += N0, write_em_outputs and with -b the posterior BAM (`threads` BGZF threads, its messages when `verbose`)
+void finish_em_sample(const EmReference& ref, int read_type, const EmArgs& a, EmSample& s, long long totNum, int MAX_ROUND,
+                      const std::string& who, int threads, bool verbose, void (*stamp)(const char*) = nullptr);
+// .theta, .model and the result rows of a sample; counts[0] already holds N0
 void write_em_outputs(const std::string& refName, const std::string& imdName, const std::string& statName,
                       const RefData& refs, const std::vector<TranscriptInfo>& transcripts, const HostModel& model,
                       std::vector<double> theta, const std::vector<double>& counts, bool appendNames);
-// gibbs_sample.cpp: the per-sample stages of rsem-run-gibbs (also used by rsem-run-gibbs-batch)
+std::string time_used_line(time_t t_start);   // "Time Used for EM.cpp : ..." (EM.cpp:673)
+
+// ---- gibbs_sample.cpp: the per-sample stages of rsem-run-gibbs, which rsem-run-gibbs-batch runs for each manifest line --
+struct GibbsArgs {   // rsem-run-gibbs's arguments after reference_name
+    std::string imdName, statName, fprior;
+    int burnin = 0, nsamples = 0, gap = 0, nThreads = 1;
+    bool hasSeed = false, hasPrior = false, quiet = false;
+    uint32_t seed = 0;
+    double pseudoC = 1.0;
+};
+// imdName statName BURNIN NSAMPLES GAP [options] (f.size() >= 5); returns "" or why they are refused
+std::string parse_gibbs_args(const std::vector<std::string>& f, GibbsArgs& a);
+void clamp_gibbs_chains(GibbsArgs& a);   // -p: at most NSAMPLES chains (with the reference's warning), at least one
+struct GibbsSample {
+    uint64_t N0 = 0, N1 = 0;
+    std::vector<uint64_t> row_ptr;   // imdName.ofg
+    std::vector<int32_t> sid;
+    std::vector<double> conprb;
+    std::vector<int32_t> init_counts, chain_samples;
+    std::vector<uint32_t> chain_seeds;
+    std::vector<double> alpha, eel, mw;
+    double totc = 0;
+};
+// load_data's imdName.ofg (Gibbs.cpp:101-137); `say` gets "Loading data is finished!"
+void load_gibbs_ofg(const GibbsArgs& a, int M, GibbsSample& s, const Say& say);
+// after the groups: load_omit_info / load_prior_info, init_model_related and init()'s chains and seeds (Gibbs.cpp:152-254)
+void load_gibbs_inputs(const GibbsArgs& a, const RefData& refs, GibbsSample& s, const Say& say);
+rsem_b200_gibbs_params gibbs_params(const GibbsArgs& a, const GibbsSample& s, const std::vector<int>& gi);
+// a sample whose chains have run: the sums of its chains, imdName.countvectors<t>, iso_res / gene_res
+void finish_gibbs_sample(const std::string& refName, const GibbsArgs& a, const GibbsSample& s, const std::vector<int>& gi,
+                         bool alleleS, const std::vector<int>& ta, const int32_t* cvs, const double* chain_acc, const Say& say);
 // load_omit_info / load_prior_info (Gibbs.cpp:152-194): init_counts (-1 = omitted), alpha and totc of a sample with N0 + N1
 // reads; returns "" or why imdName.omit or the prior file cannot be used.
 std::string gibbs_inputs(const std::string& imdName, int M, uint64_t N0, uint64_t N1, double pseudoC, const std::string* fprior,
                          std::vector<int32_t>& init_counts, std::vector<double>& alpha, double& totc);
-// imdName.countvectors<t>, one per chain (Gibbs.cpp:257-262); cvs holds the chains' vectors in chain order
-void write_countvectors(const std::string& imdName, int M, const std::vector<int32_t>& chain_samples, const int32_t* cvs);
-// release() (Gibbs.cpp:399-422): means and unbiased variances from the sums of all chains and the kept count vectors,
-// then imdName.iso_res / gene_res (and the allele file) by write_results_gibbs
-void write_gibbs_results(const std::string& refName, const std::string& imdName, int M, int NSAMPLES, const std::vector<int>& gi,
-                         bool alleleS, const std::vector<int>& ta, const int32_t* cvs, const std::vector<double>& sum_c,
-                         const std::vector<double>& sum_c2, const std::vector<double>& sum_tpm, const std::vector<double>& sum_fpkm,
-                         const std::vector<double>& sum_g2);
 void write_results_gibbs(const std::string& ref_name, const std::string& imd_name, int M, const std::vector<double>& pme_c,
                          const std::vector<double>& pme_fpkm, const std::vector<double>& pme_tpm,
                          const std::vector<double>& pve_c, const std::vector<double>& pve_c_genes,
@@ -348,11 +427,13 @@ std::vector<uint32_t> engine_seeds(uint32_t seed, int n);
 std::vector<char> slurp(const std::string& path, bool must_exist = true);
 void read_type_files(const std::string& imd_name, int tag, int read_type, std::vector<std::string>& files);
 uint32_t parse_seed(const char* s);  // digit-by-digit as EM.cpp:588-593
+double now_s();                      // steady clock, seconds
+int env_int(const char* name, int dflt);
+
+// ---- lanes.cpp: devices, and the lanes of the batch executables (one host thread, context and batch arena each) ----
 // CUDA devices of a multi-GPU run: RSEM_B200_DEVICES=0,1,... in the order given; with at most one entry there,
 // RSEM_B200_DEVICE when it is set, else that entry, else device 0
 std::vector<int> gpu_devices();
-
-// ---- lanes of the batch executables: one host thread, context and batch arena per entry of gpu_devices() ----
 // While a DieThrows(true) lives on a thread, die() and check_rc() there throw std::runtime_error instead of ending the
 // process, so that a failing lane can be reported once the other lanes have stopped.
 struct DieThrows {
@@ -385,5 +466,33 @@ class Claims {
     std::mutex mu_;
     std::string msg_;
 };
+// Runs run(lane) for every lane: the only one on this thread, or each on its own thread with die() throwing.  The first
+// failure ends the run (exit status -1) as "<tool>: device D, <where>: <what>" once every lane has stopped; a Lane
+// needs `device` and `where` (what it is working on) for it.
+template <class Lane, class Run>
+void run_lanes(const char* tool, std::vector<Lane>& lanes, Claims& claims, Run run) {
+    if (lanes.size() == 1) return run(lanes[0]);
+    auto lane_main = [&](Lane& L) {
+        DieThrows throws(true);
+        try {
+            run(L);
+        } catch (const std::exception& e) {
+            claims.fail(std::string(tool) + ": device " + std::to_string(L.device) + ", " + L.where + ": " + e.what());
+        }
+    };
+    std::vector<std::thread> pool;
+    for (size_t k = 1; k < lanes.size(); ++k) pool.emplace_back(lane_main, std::ref(lanes[k]));
+    lane_main(lanes[0]);
+    for (auto& th : pool) th.join();
+    if (claims.failed()) die(claims.message());
+}
+// The non-empty lines of a manifest: 1-based line number and whitespace-separated fields
+struct ManifestLine {
+    int no;
+    std::vector<std::string> f;
+};
+std::vector<ManifestLine> manifest_lines(const std::string& path);
+[[noreturn]] void refuse(const std::string& manifest, int no, const std::string& why);   // "<manifest> line N: why"
+std::string sample_at(const std::string& name, const std::string& manifest, int no);     // "sample X (<manifest> line N)"
 
 }  // namespace host

@@ -20,16 +20,13 @@
 // have finished their current samples.  Standard output has one block per sample, in manifest order.
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <cstdlib>
 #include <cstring>
-#include <ctime>
 #include <deque>
 #include <future>
 #include <map>
 #include <memory>
 #include <mutex>
-#include <sstream>
 #include <thread>
 
 #include "host.hpp"
@@ -38,26 +35,13 @@ using namespace host;
 
 namespace {
 
-struct Line {
+struct Line : GibbsArgs {
     int no = 0;   // 1-based line number in the manifest
-    std::string imdName, statName, fprior;
-    int burnin = 0, nsamples = 0, gap = 0, nThreads = 1;
-    bool hasSeed = false, hasPrior = false;
-    uint32_t seed = 0;
-    double pseudoC = 1.0;
 };
 
 // a loaded sample, from its .ofg to its written outputs
-struct Sample {
+struct Sample : GibbsSample {
     size_t idx = 0;
-    uint64_t N0 = 0, N1 = 0;
-    std::vector<uint64_t> row_ptr;
-    std::vector<int32_t> sid;
-    std::vector<double> conprb;
-    std::vector<int32_t> init_counts, chain_samples;
-    std::vector<uint32_t> chain_seeds;
-    std::vector<double> alpha, eel, mw;
-    double totc = 0;
 };
 
 void usage() {
@@ -68,41 +52,17 @@ void usage() {
     exit(-1);
 }
 
-[[noreturn]] void refuse(const std::string& manifest, int no, const std::string& why) {
-    die(manifest + " line " + std::to_string(no) + ": " + why);
-}
-
-double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
 // every manifest line is checked before the context is created and before any output is written
 std::vector<Line> read_manifest(const std::string& path, int M) {
-    std::vector<char> buf = slurp(path);
-    std::string text(buf.begin(), buf.end());
-    std::istringstream in(text);
     std::vector<Line> lines;
     std::map<std::string, int> seen;
-    std::string raw;
-    for (int no = 1; std::getline(in, raw); ++no) {
-        std::istringstream ls(raw);
-        std::vector<std::string> f;
-        for (std::string w; ls >> w;) f.push_back(w);
-        if (f.empty()) continue;
-        if (f.size() < 5) refuse(path, no, "too few fields (imdName statName BURNIN NSAMPLES GAP [options])");
+    for (const ManifestLine& ml : manifest_lines(path)) {
+        const int no = ml.no;
+        if (ml.f.size() < 5) refuse(path, no, "too few fields (imdName statName BURNIN NSAMPLES GAP [options])");
         Line l;
         l.no = no;
-        l.imdName = f[0];
-        l.statName = f[1];
-        l.burnin = atoi(f[2].c_str());
-        l.nsamples = atoi(f[3].c_str());
-        l.gap = atoi(f[4].c_str());
-        for (size_t i = 5; i < f.size(); ++i) {   // the option rules of rsem-run-gibbs
-            if (f[i] == "-p" && i + 1 < f.size()) l.nThreads = atoi(f[i + 1].c_str());
-            if (f[i] == "--seed" && i + 1 < f.size()) { l.hasSeed = true; l.seed = parse_seed(f[i + 1].c_str()); }
-            if (f[i] == "--pseudo-count" && i + 1 < f.size()) l.pseudoC = atof(f[i + 1].c_str());
-            if (f[i] == "--prior" && i + 1 < f.size()) { l.hasPrior = true; l.fprior = f[i + 1]; }
-        }
-        if (!(l.nsamples > 1)) refuse(path, no, "NSAMPLES must be larger than 1, otherwise the posterior variance cannot be calculated!");
-        if (l.gap < 1) refuse(path, no, "GAP must be at least 1!");
+        const std::string why = parse_gibbs_args(ml.f, l);
+        if (!why.empty()) refuse(path, no, why);
         auto it = seen.find(l.imdName);
         if (it != seen.end()) refuse(path, no, "its outputs collide with line " + std::to_string(it->second) + " (same imdName)");
         seen[l.imdName] = no;
@@ -130,11 +90,7 @@ std::vector<Line> read_manifest(const std::string& path, int M) {
             if (fi) fclose(fi);
             if (!ok) refuse(path, no, "cannot read or parse " + l.statName + ".model");
         }
-        if (l.nThreads > l.nsamples) {
-            l.nThreads = l.nsamples;
-            fprintf(stderr, "Warning: Number of samples is less than number of threads! Change the number of threads to %d!\n", l.nThreads);
-        }
-        if (l.nThreads < 1) l.nThreads = 1;
+        clamp_gibbs_chains(l);
         lines.push_back(l);
     }
     return lines;
@@ -152,7 +108,7 @@ struct Phases {
 struct Run {
     std::string refName, manifest;
     bool verbose = true;
-    int M = 0, m = 0;
+    int M = 0;
     size_t acc_per = 0;
     bool alleleS = false;
     std::vector<Line> lines;
@@ -178,7 +134,7 @@ struct Lane {
 void run_lane(Run& R, Lane& L, Claims& claims) {
     const std::vector<Line>& lines = R.lines;
     const std::string& refName = R.refName;
-    const int M = R.M, m = R.m;
+    const int M = R.M;
     const size_t acc_per = R.acc_per;
     const RefData& refs = R.refs;
     const std::vector<int>& gi = R.gi;
@@ -193,9 +149,7 @@ void run_lane(Run& R, Lane& L, Claims& claims) {
         std::lock_guard<std::mutex> g(R.block_mu);
         R.block[i] += s;
     };
-    auto sample_at = [&](size_t i) {
-        return "sample " + lines[i].imdName + " (" + R.manifest + " line " + std::to_string(lines[i].no) + ")";
-    };
+    auto sample_of = [&](size_t i) { return sample_at(lines[i].imdName, R.manifest, lines[i].no); };
     // a cooperative launch: one at a time per device
     auto launch = [&](const auto& run) {
         std::lock_guard<std::mutex> g(*L.launch_mu);
@@ -204,58 +158,22 @@ void run_lane(Run& R, Lane& L, Claims& claims) {
         L.launches.emplace_back(t0, now_s());
     };
 
-    // a sample's inputs (rsem-run-gibbs's load_data, load_omit_info / load_prior_info, init_model_related, init)
+    // a sample's inputs, with the progress lines of rsem-run-gibbs; the reference and its groups are the run's
     auto load = [&](size_t i) {
         DieThrows throws(L.isolated);
-        const Line& l = lines[i];
         auto s = std::make_unique<Sample>();
         s->idx = i;
-        load_ofg(l.imdName + ".ofg", M, s->N0, s->row_ptr, s->sid, s->conprb);
-        s->N1 = s->row_ptr.size() - 1;
-        const std::string why = gibbs_inputs(l.imdName, M, s->N0, s->N1, l.pseudoC, l.hasPrior ? &l.fprior : nullptr, s->init_counts,
-                                             s->alpha, s->totc);
-        if (!why.empty()) die(why);
-        int model_type = 0;
-        LenDistH gld;
-        HostModel::read_for_gibbs(l.statName + ".model", M, model_type, gld, s->mw);
-        calc_eel(refs, gld, s->eel);
-        s->chain_seeds = engine_seeds(l.hasSeed ? l.seed : (uint32_t)time(NULL), l.nThreads);
-        s->chain_samples.resize(l.nThreads);
-        const int quotient = l.nsamples / l.nThreads, left = l.nsamples % l.nThreads;
-        for (int t = 0; t < l.nThreads; ++t) s->chain_samples[t] = quotient + (t < left ? 1 : 0);
+        auto say_i = [&](const std::string& x) { say(i, x); };
+        say_i("Refs.loadRefs finished!\n");
+        load_gibbs_ofg(lines[i], M, *s, say_i);
+        say_i("Loading group information is finished!\n");
+        load_gibbs_inputs(lines[i], refs, *s, say_i);
         return s;
     };
-    auto params_of = [&](const Sample& s) {
-        const Line& l = lines[s.idx];
-        rsem_b200_gibbs_params gp;
-        memset(&gp, 0, sizeof gp);
-        gp.M = M; gp.burnin = l.burnin; gp.gap = l.gap; gp.n_chains = l.nThreads;
-        gp.chain_samples = s.chain_samples.data();
-        gp.chain_seeds = s.chain_seeds.data();
-        gp.n0 = (double)s.N0;
-        gp.init_counts = s.init_counts.data();
-        gp.pseudo_counts = s.alpha.data();
-        gp.totc = s.totc;
-        gp.eel = s.eel.data();
-        gp.mw = s.mw.data();
-        gp.n_genes = m;
-        gp.gene_start = gi.data();
-        return gp;
-    };
-    // a sample whose chains have run: the sums of its chains, countvectors<t>, iso_res / gene_res (rsem-run-gibbs from
-    // rsem_b200_gibbs_sum_chains on)
+    // a sample whose chains have run
     auto finish = [&](const Sample& s, const std::vector<int32_t>& cvs, const std::vector<double>& chain_acc) {
-        const Line& l = lines[s.idx];
-        std::vector<double> sum_c(M + 1), sum_c2(M + 1), sum_tpm(M + 1), sum_fpkm(M + 1), sum_g2(m);
-        rsem_b200_gibbs_out go;
-        go.count_vectors = nullptr;
-        go.sum_c = sum_c.data(); go.sum_c2 = sum_c2.data(); go.sum_tpm = sum_tpm.data(); go.sum_fpkm = sum_fpkm.data();
-        go.sum_gene_c2 = sum_g2.data();
-        const rsem_b200_gibbs_params gp = params_of(s);
-        check_rc(rsem_b200_gibbs_sum_chains(&gp, chain_acc.data(), &go), "gibbs_sum_chains");
-        write_countvectors(l.imdName, M, s.chain_samples, cvs.data());
-        say(s.idx, "Gibbs finished!\n");
-        write_gibbs_results(refName, l.imdName, M, l.nsamples, gi, alleleS, ta, cvs.data(), sum_c, sum_c2, sum_tpm, sum_fpkm, sum_g2);
+        finish_gibbs_sample(refName, lines[s.idx], s, gi, alleleS, ta, cvs.data(), chain_acc.data(),
+                            [&](const std::string& x) { say(s.idx, x); });
         say(s.idx, "Gibbs based expression values are written!\n");
     };
 
@@ -300,7 +218,7 @@ void run_lane(Run& R, Lane& L, Claims& claims) {
                 t_write[w] += now_s() - t1;
             } catch (...) {
                 std::lock_guard<std::mutex> g(copy_mu);
-                if (!failed) { failed = std::current_exception(); L.where = sample_at(todo[k].second->idx); }
+                if (!failed) { failed = std::current_exception(); L.where = sample_of(todo[k].second->idx); }
                 next = todo.size();
             }
         };
@@ -329,13 +247,12 @@ void run_lane(Run& R, Lane& L, Claims& claims) {
     };
     for (top_up(); !loads.empty(); top_up()) {
         const size_t i = loads.front().first;
-        L.where = sample_at(i);
+        L.where = sample_of(i);
         const Line& l = lines[i];
         const double t_load = now_s();
         std::unique_ptr<Sample> s = loads.front().second.get();
         loads.pop_front();
-        say(i, "Refs.loadRefs finished!\nLoading data is finished!\nLoading group information is finished!\nGibbs started!\nInitialization finished!\n");
-        const rsem_b200_gibbs_params gp = params_of(*s);
+        const rsem_b200_gibbs_params gp = gibbs_params(l, *s, gi);
         int32_t slot = -1;
         int rc = rsem_b200_gibbs_batch_add(batch, s->N1, s->sid.size(), s->row_ptr.data(), s->sid.data(), s->conprb.data(), &gp, &slot);
         ph.load += now_s() - t_load;
@@ -383,9 +300,8 @@ int main(int argc, char* argv[]) {
         if (!strcmp(argv[i], "-q")) R.verbose = false;
     g_verbose = false;   // the messages of the shared loaders and writers go into the samples' blocks instead
     {   // as rsem-run-gibbs: file parsing and writing use the host's cores
-        const char* e = getenv("RSEM_B200_IO_THREADS");
         const unsigned hw = std::thread::hardware_concurrency();
-        g_io_threads = e ? atoi(e) : (int)std::min<unsigned>(hw ? hw : 1, 32);
+        g_io_threads = env_int("RSEM_B200_IO_THREADS", (int)std::min<unsigned>(hw ? hw : 1, 32));
     }
     load_refs(R.refName + ".seq", false, R.refs);
     R.M = R.refs.M;
@@ -394,13 +310,12 @@ int main(int argc, char* argv[]) {
     const std::vector<int> devices = gpu_devices();
     std::future<LaneContexts> ctx_future = std::async(std::launch::async, open_lanes, devices);
     load_groups(R.refName + ".grp", R.gi);
-    R.m = (int)R.gi.size() - 1;
     R.alleleS = load_allele_groups(R.refName, R.gt, R.ta);
-    R.acc_per = 4 * ((size_t)R.M + 1) + (size_t)R.m;
+    R.acc_per = 4 * ((size_t)R.M + 1) + R.gi.size() - 1;
     R.block.resize(R.lines.size());
     if (R.verbose)
         for (size_t i = 0; i < R.lines.size(); ++i)
-            R.block[i] = "== sample " + R.lines[i].imdName + " (" + R.manifest + " line " + std::to_string(R.lines[i].no) + ")\n";
+            R.block[i] = "== " + sample_at(R.lines[i].imdName, R.manifest, R.lines[i].no) + "\n";
 
     std::vector<Lane> lanes(devices.size());
     std::map<int, std::mutex> launch_mu;
@@ -416,23 +331,7 @@ int main(int argc, char* argv[]) {
         }
     }
     Claims claims(R.lines.size());
-    if (lanes.size() == 1) {
-        run_lane(R, lanes[0], claims);
-    } else {
-        auto lane_main = [&](Lane& L) {
-            DieThrows throws(true);
-            try {
-                run_lane(R, L, claims);
-            } catch (const std::exception& e) {
-                claims.fail("rsem-run-gibbs-batch: device " + std::to_string(L.device) + ", " + L.where + ": " + e.what());
-            }
-        };
-        std::vector<std::thread> pool;
-        for (size_t k = 1; k < lanes.size(); ++k) pool.emplace_back(lane_main, std::ref(lanes[k]));
-        lane_main(lanes[0]);
-        for (auto& th : pool) th.join();
-        if (claims.failed()) die(claims.message());
-    }
+    run_lanes("rsem-run-gibbs-batch", lanes, claims, [&](Lane& L) { run_lane(R, L, claims); });
     if (getenv("RSEM_B200_TIMING")) {
         Phases ph;   // the totals
         for (const Lane& L : lanes) {

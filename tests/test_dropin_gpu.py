@@ -166,6 +166,19 @@ def test_bam_of_a_sample_without_alignable_reads(workdir):
     assert filecmp.cmp(f"{base}/aln.sam", f"{base}/s.transcript.bam", shallow=False)
 
 
+def test_em_runs_on_the_listed_device(workdir):
+    """RSEM_B200_DEVICES=99 (one entry, RSEM_B200_DEVICE unset) names rsem-run-em's device as it does every other tool's: the
+    CUDA runtime refuses the ordinal, so the run ends naming ctx_create before any output is written"""
+    import subprocess
+    base = rf.gen_dataset(str(workdir / "device99"), read_type=0, M=30, N1=200, N0=10)
+    env = dict(os.environ, RSEM_B200_DEVICES="99")
+    env.pop("RSEM_B200_DEVICE", None)
+    p = subprocess.run([os.path.join(rf.BIN_DIR, "rsem-run-em"), "ref/r", "0", "s", "s.temp/s", "s.stat/s"], cwd=base, env=env,
+                       capture_output=True, text=True)
+    assert p.returncode == 255 and "ctx_create" in p.stderr, p.stderr
+    assert not os.path.exists(f"{base}/s.stat/s.theta")
+
+
 def test_em_two_gpus_matches_reference(workdir, live_ref):
     """RSEM_B200_DEVICES=0,1: reads sharded over two GPUs (same rule as the reference's threads), counts and model
     statistics summed with ncclAllReduce inside the library.  Needs a machine with >= 2 GPUs."""

@@ -108,9 +108,10 @@ def test_batch_matches_single_sample_runs(tmp_path, built, name, rounds):
         s = rf.clone(d, d + "_single")
         singles.append((s, _single(s, os.path.basename(d), rt, extra, rounds)))
     with open(tmp_path / "manifest", "w") as f:
-        for d, extra in samples:
+        for k, (d, extra) in enumerate(samples):
             b = os.path.basename(d)
-            f.write(" ".join([f"{b}/s", f"{b}/s.temp/s", f"{b}/s.stat/s", *extra]) + "\n\n")
+            run_opts = ["-q", "-p", "3"] if k == 3 else []   # the run's options: a manifest line's are ignored
+            f.write(" ".join([f"{b}/s", f"{b}/s.temp/s", f"{b}/s.stat/s", *extra, *run_opts]) + "\n\n")
     env = dict(os.environ)
     if rounds is not None:
         env["RSEM_MAX_ROUND"], env["RSEM_MIN_ROUND"] = str(rounds), str(min(20, rounds))
