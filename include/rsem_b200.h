@@ -368,6 +368,32 @@ typedef struct rsem_b200_sim_stats {
  * NULL, the phase times; frees the state                                                                     */
 int rsem_b200_sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 
+/* ---- read simulation over several contexts (RSEM_B200_DEVICES) ----------------------------------------------------
+ * The same reads as rsem_b200_sim_begin / _next / _end on one context for the same params, byte for byte.  Stream
+ * window w (words [w W, (w + 1) W + L)) belongs to context w mod n: each context generates the W + L words of its
+ * windows and jumps its mt19937 state ahead to its next one (rsem_b200_mt19937_jump's scheme, on the device).  The
+ * attempt lengths of all windows are worked out side by side; the chain of attempts crosses the windows in order, each
+ * window's entry point handed from one context to the next.  n >= 2; contexts may share a device.  The handle does not
+ * own the contexts; each holds its part of the run as after rsem_b200_sim_begin until rsem_b200_sim_end_devices.     */
+typedef struct rsem_b200_sim_multi rsem_b200_sim_multi;
+int rsem_b200_sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_params* params,
+                                rsem_b200_sim_multi** out);
+/* as rsem_b200_sim_next: chunks in read order, each valid until the second following call */
+int rsem_b200_sim_next_devices(rsem_b200_sim_multi* multi, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
+typedef struct rsem_b200_sim_devices_stats {
+    rsem_b200_sim_stats sum;  /* summed over the contexts; generate_ms excludes the jumps                       */
+    double jump_ms;           /* mt19937 jumps between a context's windows (on the generator streams, overlapped) */
+    double handoff_ms;        /* host time waiting for each window's chain resolution, whose exit is the next
+                                 window's entry point                                                         */
+} rsem_b200_sim_devices_stats;
+/* counts and failed attempts summed over the contexts, stats (may be NULL), per_device (n entries, may be NULL: each
+ * context's own phases); frees every context's simulation state and the handle                             */
+int rsem_b200_sim_end_devices(rsem_b200_sim_multi* multi, double* counts, uint64_t* resim,
+                              rsem_b200_sim_devices_stats* stats, rsem_b200_sim_stats* per_device);
+/* Device-free: state_out = the boost::mt19937 state after J draws from state_in.  state[0..623] are the words,
+ * state[624] the index (624: twist before the next draw).  Runs on the host; needs no GPU.                     */
+int rsem_b200_mt19937_jump(const uint32_t state_in[625], uint64_t J, uint32_t state_out[625]);
+
 /* ---- rsem-calculate-credibility-intervals, Phase II (K8, ci_kernels.cu) ------------------------------------------------
  * Replaces the reference's temp-file transpose (Buffer.h:41-80, calcCI.cpp:302-305) and calculate_credibility_intervals
  * (calcCI.cpp:286-508).  The caller draws the samples (calcCI.cpp:93-164) and pushes each one's TPM row and l_bar at a

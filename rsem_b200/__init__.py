@@ -5,4 +5,4 @@ drop-in executables `bin/rsem-run-em` / `bin/rsem-run-gibbs` (C++ hosts in rsem_
 Python package is a thin ctypes mirror of the C ABI used by the tests and by bench.py; it contains
 no arithmetic of its own and no CPU fallback.
 """
-from .capi import Batch, Context, GibbsBatch, Lib, RsemB200Error, load_library  # noqa: F401
+from .capi import Batch, Context, GibbsBatch, Lib, RsemB200Error, SimDevices, load_library  # noqa: F401

@@ -78,6 +78,10 @@ class SimStats(C.Structure):
                 ("copy_ms", C.c_double), ("words", C.c_uint64), ("windows", C.c_uint64)]
 
 
+class SimDevicesStats(C.Structure):
+    _fields_ = [("sum", SimStats), ("jump_ms", C.c_double), ("handoff_ms", C.c_double)]
+
+
 class CiParams(C.Structure):
     _fields_ = [("M", C.c_int32), ("n_genes", C.c_int32), ("gene_start", C.POINTER(C.c_int32)),
                 ("n_isoforms", C.c_int32), ("n_parts", C.c_int32), ("isoform_start", C.POINTER(C.c_int32)),
@@ -146,6 +150,7 @@ SYMBOLS = [
     "rsem_b200_batch_final", "rsem_b200_batch_remove", "rsem_b200_batch_timing", "rsem_b200_gibbs_batch_create",
     "rsem_b200_gibbs_batch_destroy", "rsem_b200_gibbs_batch_sample_bytes", "rsem_b200_gibbs_batch_add",
     "rsem_b200_gibbs_batch_run", "rsem_b200_gibbs_batch_result", "rsem_b200_gibbs_batch_clear",
+    "rsem_b200_sim_begin_devices", "rsem_b200_sim_next_devices", "rsem_b200_sim_end_devices", "rsem_b200_mt19937_jump",
 ]
 
 RSEM_B200_ERR_ARG = 2
@@ -199,6 +204,14 @@ class Lib:
         """out's sums = the params.n_chains per-chain blocks of chain_acc added up in chain order"""
         chain_acc = _arr(chain_acc, np.float64)
         self.check(self.dll.rsem_b200_gibbs_sum_chains(C.byref(params), _dp(chain_acc), C.byref(out)))
+
+    def mt19937_jump(self, state, J: int) -> np.ndarray:
+        """the boost::mt19937 state (625 uint32: the words, then the index) after J draws from state; host only"""
+        state = _arr(state, np.uint32)
+        assert state.shape == (625,)
+        out = np.zeros(625, np.uint32)
+        self.check(self.dll.rsem_b200_mt19937_jump(_p(state, C.c_uint32), C.c_uint64(J), _p(out, C.c_uint32)))
+        return out
 
     def comm_unique_id(self) -> bytes:
         buf = C.create_string_buffer(128)
@@ -487,6 +500,36 @@ class Context:
 
     def set_estep_variant(self, v: int):
         self.lib.check(self.lib.dll.rsem_b200_set_estep_variant(self._h, C.c_int32(v)))
+
+
+class SimDevices:
+    """rsem-simulate-reads over several contexts (rsem_b200_sim_*_devices): the reads of Context.sim_* on one context"""
+
+    def __init__(self, ctxs, params: SimParams):
+        """params' arrays must stay alive until the constructor returns (they are copied to the devices)"""
+        self.lib = ctxs[0].lib
+        self.ctxs = list(ctxs)
+        self._h = C.c_void_p()
+        arr = (C.c_void_p * len(ctxs))(*[c._h.value for c in ctxs])
+        self.lib.check(self.lib.dll.rsem_b200_sim_begin_devices(arr, C.c_int(len(ctxs)), C.byref(params), C.byref(self._h)))
+
+    def next(self):
+        """-> (n_reads, [mate 1 text, mate 2 text]) of the next chunk; n_reads == 0 after the last one"""
+        text = (C.c_void_p * 2)()
+        nbytes = (C.c_uint64 * 2)()
+        n = C.c_uint64(0)
+        self.lib.check(self.lib.dll.rsem_b200_sim_next_devices(self._h, text, nbytes, C.byref(n)))
+        return n.value, [C.string_at(text[i], nbytes[i]) if text[i] else b"" for i in range(2)]
+
+    def end(self, M: int):
+        """-> (counts per sid, M + 1 doubles; failed attempts; SimDevicesStats; [SimStats per context])"""
+        counts = np.zeros(M + 1, np.float64)
+        resim = C.c_uint64(0)
+        stats = SimDevicesStats()
+        per = (SimStats * len(self.ctxs))()
+        h, self._h = self._h, C.c_void_p()
+        self.lib.check(self.lib.dll.rsem_b200_sim_end_devices(h, _dp(counts), C.byref(resim), C.byref(stats), per))
+        return counts, resim.value, stats, list(per)
 
 
 class Batch:

@@ -902,8 +902,8 @@ int rsem_b200_gibbs_batch_clear(rsem_b200_gibbs_batch* b) {
     return 0;
 }
 
-int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
-    RB_ARG(c && p, "NULL argument");
+namespace {
+int check_sim_params(const rsem_b200_sim_params* p) {
     RB_ARG(p->model_type >= 0 && p->model_type <= 3 && p->M >= 1, "bad model type or M");
     RB_ARG(p->theta_cdf && p->gld.cdf && p->profile_cdf && p->noise_cdf && p->seq_off && p->seq && p->tot_len &&
                p->full_len, "NULL table");
@@ -912,6 +912,13 @@ int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
     RB_ARG(!p->has_mld || (p->mld.cdf && p->mld.span == p->mld.ub - p->mld.lb && p->mld.span >= 1), "bad mld");
     RB_ARG(!p->est_rspd || (p->rspd_off && p->rspd_cdf), "estRSPD needs rspd_off / rspd_cdf");
     RB_ARG(!(p->model_type & 1) || (p->qd_init_cdf && p->qd_tran_cdf && p->pro_rows == 100), "Q models need QualDist");
+    return 0;
+}
+}  // namespace
+
+int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
+    RB_ARG(c && p, "NULL argument");
+    if (int rc = check_sim_params(p)) return rc;
     RB_CUDA(cudaSetDevice(c->device));
     return sim_begin(c, p);
 }
@@ -926,6 +933,29 @@ int rsem_b200_sim_end(rsem_b200_ctx* c, double* counts, uint64_t* resim, rsem_b2
     RB_ARG(c, "NULL argument");
     RB_CUDA(cudaSetDevice(c->device));
     return sim_end(c, counts, resim, stats);
+}
+
+int rsem_b200_sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_params* p,
+                                rsem_b200_sim_multi** out) {
+    RB_ARG(ctxs && p && out, "NULL argument");
+    RB_ARG(n >= 2, "sim_begin_devices needs at least two contexts (one context: rsem_b200_sim_begin)");
+    for (int i = 0; i < n; ++i) RB_ARG(ctxs[i], "NULL context");
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < i; ++j) RB_ARG(ctxs[i] != ctxs[j], "a context is listed twice");
+    if (int rc = check_sim_params(p)) return rc;
+    *out = nullptr;
+    return sim_begin_devices(ctxs, n, p, out);
+}
+
+int rsem_b200_sim_next_devices(rsem_b200_sim_multi* m, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {
+    RB_ARG(m && text && bytes && n_reads, "NULL argument");
+    return sim_next_devices(m, text, bytes, n_reads);
+}
+
+int rsem_b200_sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rsem_b200_sim_devices_stats* stats,
+                              rsem_b200_sim_stats* per_device) {
+    RB_ARG(m, "NULL argument");
+    return sim_end_devices(m, counts, resim, stats, per_device);
 }
 
 int rsem_b200_ci_begin(rsem_b200_ctx* c, const rsem_b200_ci_params* p) {

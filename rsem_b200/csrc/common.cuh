@@ -386,6 +386,26 @@ int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p);
 int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
 int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 void sim_free(rsem_b200_ctx* ctx);
+int sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_params* p, rsem_b200_sim_multi** out);
+int sim_next_devices(rsem_b200_sim_multi* m, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
+int sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rsem_b200_sim_devices_stats* stats,
+                    rsem_b200_sim_stats* per_device);
+
+// mt_jump.cpp: MT19937 jump-ahead.  A jump of J draws from a state with index idx moves its array by `blocks` twists
+// and leaves index `idx`; blocks >= 1 is computed as one twist, then g(T) with g = x^(624 (blocks - 1)) mod p.
+constexpr int kMtPolyWords = 312;   // 64-bit words of a polynomial of degree < 19937
+constexpr int kMtJumpBlocks = 32;   // 624-coefficient blocks of such a polynomial (32 x 624 >= 19937)
+constexpr int kMtBlockWords = 20;   // 32-bit words per block (624 bits, padded)
+struct MtJumpPlan {
+    uint32_t idx;
+    uint64_t blocks;
+};
+MtJumpPlan mt_jump_plan(uint32_t idx, uint64_t J);
+// x^J mod p(x), bit i = coefficient of x^i; false when p could not be found
+bool mt_jump_poly(uint64_t J, uint64_t out[kMtPolyWords]);
+// poly cut into kMtJumpBlocks blocks of 624 bits (kMtBlockWords words each); returns the number of blocks up to the
+// last nonzero one
+int mt_jump_blocks(const uint64_t poly[kMtPolyWords], uint32_t blocks[kMtJumpBlocks * kMtBlockWords]);
 
 // ci_kernels.cu
 int ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* p);

@@ -26,10 +26,21 @@
 #include <thrust/iterator/counting_iterator.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "common.cuh"
+
+// several contexts, each owning every G-th window (sim_begin_devices)
+struct rsem_b200_sim_multi {
+    std::vector<rsem_b200_ctx*> ctx;
+    uint64_t N = 0, done = 0;
+    uint64_t window = 0;   // the window sim_next_devices resolves next, on context window % G
+    uint32_t entry = 0;    // its entry point
+    double handoff_ms = 0;
+};
 
 namespace rsem_b200 {
 
@@ -190,6 +201,30 @@ __device__ bool attempt(const SimTables& t, Cur& c, Head& h, char* seq_out[2], c
 }
 
 // ---- 1. the mt19937 stream ------------------------------------------------------------------------------------------
+// boost's twist of the 624 words in shared memory, thread k of 624 owning word k.  Phase i uses mt[i + 1] (old) and
+// mt[i + 397 mod 624], new from phase i - 1 for i >= 227.  Ends with a barrier.
+__device__ __forceinline__ void mt_twist(uint32_t* mt, int k) {
+    auto twist = [&](int i, uint32_t next) {
+        const uint32_t y = (mt[i] & 0x80000000u) | (next & 0x7fffffffu);
+        return mt[(i + 397) % kMtN] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
+    };
+    uint32_t v = 0;
+    if (k < 227) v = twist(k, mt[k + 1]);
+    __syncthreads();
+    if (k < 227) mt[k] = v;
+    __syncthreads();
+    if (k >= 227 && k < 454) v = twist(k, mt[k + 1]);
+    __syncthreads();
+    if (k >= 227 && k < 454) mt[k] = v;
+    __syncthreads();
+    if (k >= 454 && k < 623) v = twist(k, mt[k + 1]);
+    __syncthreads();
+    if (k >= 454 && k < 623) mt[k] = v;
+    __syncthreads();
+    if (k == 623) mt[k] = twist(k, mt[0]);
+    __syncthreads();
+}
+
 // state[0..623] = the engine's words, state[624] = its index (boost: i == n means "twist before the next draw")
 __global__ void __launch_bounds__(kMtN) sim_mt_kernel(uint32_t* __restrict__ state, uint32_t* __restrict__ out, uint64_t n) {
     __shared__ uint32_t mt[kMtN];
@@ -200,28 +235,9 @@ __global__ void __launch_bounds__(kMtN) sim_mt_kernel(uint32_t* __restrict__ sta
     __syncthreads();
     int idx = idx_s;
     uint64_t done = 0;
-    auto twist = [&](int i, uint32_t next) {
-        const uint32_t y = (mt[i] & 0x80000000u) | (next & 0x7fffffffu);
-        return mt[(i + 397) % kMtN] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-    };
     while (done < n) {
         if (idx >= kMtN) {
-            // phase i uses mt[i + 1] (old) and mt[i + 397 mod 624], new from phase i - 1 for i >= 227
-            uint32_t v = 0;
-            if (k < 227) v = twist(k, mt[k + 1]);
-            __syncthreads();
-            if (k < 227) mt[k] = v;
-            __syncthreads();
-            if (k >= 227 && k < 454) v = twist(k, mt[k + 1]);
-            __syncthreads();
-            if (k >= 227 && k < 454) mt[k] = v;
-            __syncthreads();
-            if (k >= 454 && k < 623) v = twist(k, mt[k + 1]);
-            __syncthreads();
-            if (k >= 454 && k < 623) mt[k] = v;
-            __syncthreads();
-            if (k == 623) mt[k] = twist(k, mt[0]);
-            __syncthreads();
+            mt_twist(mt, k);
             idx = 0;
         }
         const uint64_t take = min((uint64_t)(kMtN - idx), n - done);
@@ -239,6 +255,54 @@ __global__ void __launch_bounds__(kMtN) sim_mt_kernel(uint32_t* __restrict__ sta
     __syncthreads();
     state[k] = mt[k];
     if (k == 0) state[kMtN] = (uint32_t)idx;
+}
+
+// The jump of several devices' generators (mt_jump.cpp has the method and its host twin).  The state's array moves
+// one twist, to S, then by g(T) S with g cut into blocks h_b of 624 coefficients:
+// conv[b][j] = sum_i h_b,i s_{i + j} over the 1248 words s = (S, twist(S)), one CTA per block (they are independent);
+__global__ void __launch_bounds__(kMtN) sim_mt_jump_conv_kernel(const uint32_t* __restrict__ state,
+                                                                const uint32_t* __restrict__ poly,
+                                                                uint32_t* __restrict__ conv) {
+    __shared__ uint32_t s[2 * kMtN];
+    __shared__ uint32_t h[kMtBlockWords];
+    const int k = threadIdx.x, b = blockIdx.x;
+    s[k] = state[k];
+    if (k < kMtBlockWords) h[k] = poly[b * kMtBlockWords + k];
+    __syncthreads();
+    mt_twist(s, k);
+    s[kMtN + k] = s[k];
+    __syncthreads();
+    mt_twist(s + kMtN, k);
+    uint32_t acc = 0;
+#pragma unroll 1
+    for (int wi = 0; wi < kMtBlockWords; ++wi) {
+        const uint32_t w = h[wi];
+        const int base = wi * 32 + k;
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+            if (wi * 32 + i < kMtN) acc ^= s[base + i] & (0u - ((w >> i) & 1u));
+    }
+    conv[b * kMtN + k] = acc;
+}
+
+// then Horner's rule over the blocks, acc = twist(acc) ^ conv[b] from the last block down, and the new index.
+// nb == 0: the array stays, only the index moves.
+__global__ void __launch_bounds__(kMtN) sim_mt_jump_horner_kernel(uint32_t* __restrict__ state,
+                                                                  const uint32_t* __restrict__ conv, int nb,
+                                                                  uint32_t idx) {
+    __shared__ uint32_t mt[kMtN];
+    const int k = threadIdx.x;
+    if (nb > 0) {
+        mt[k] = conv[(nb - 1) * kMtN + k];
+        __syncthreads();
+        for (int b = nb - 2; b >= 0; --b) {
+            mt_twist(mt, k);
+            mt[k] ^= conv[b * kMtN + k];
+            __syncthreads();
+        }
+        state[k] = mt[k];
+    }
+    if (k == 0) state[kMtN] = idx;
 }
 
 // ---- 2. attempt lengths -----------------------------------------------------------------------------------------------
@@ -436,6 +500,18 @@ struct SimState {
     int slot = 0;
     double* counts = nullptr;
     rsem_b200_sim_stats stats{};
+
+    // one of G >= 2 contexts of sim_begin_devices: `window` counts this context's own windows, each W + L fresh words
+    // followed by a jump to the start of its next one
+    int G = 1;
+    uint64_t gen_pos = 0;            // stream position of the generator's state once the enqueued work has run
+    uint64_t step_blocks = 0;        // the jump between windows moves the array step_blocks or step_blocks + 1 twists
+    uint32_t* step_poly[2] = {nullptr, nullptr};  // kMtJumpBlocks x kMtBlockWords each, for those two
+    int step_nb[2] = {0, 0};
+    uint32_t* jump_conv = nullptr;   // kMtJumpBlocks x 624
+    cudaEvent_t jump_ev[2] = {nullptr, nullptr};       // per buffer: generation done, jump starts
+    cudaEvent_t prep_ev[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // per buffer: attempt lengths + tables
+    double jump_ms = 0;
 };
 
 void sim_free(rsem_b200_ctx* ctx) {
@@ -449,6 +525,8 @@ void sim_free(rsem_b200_ctx* ctx) {
     for (auto& e : s->gen_ev) for (cudaEvent_t x : e) if (x) cudaEventDestroy(x);
     for (cudaEvent_t x : s->used_ev) if (x) cudaEventDestroy(x);
     for (cudaEvent_t x : s->ph_ev) if (x) cudaEventDestroy(x);
+    for (cudaEvent_t x : s->jump_ev) if (x) cudaEventDestroy(x);
+    for (auto& e : s->prep_ev) for (cudaEvent_t x : e) if (x) cudaEventDestroy(x);
     if (s->gen_stream) cudaStreamDestroy(s->gen_stream);
     delete s;
     ctx->sim = nullptr;
@@ -488,7 +566,11 @@ float elapsed(cudaEvent_t a, cudaEvent_t b) {
 
 }  // namespace
 
-int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p) {
+namespace {
+
+// the tables, buffers, streams and events of a run; the generator's state is boost::mt19937(seed), or `state` (625
+// words) when given
+int sim_setup(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p, const uint32_t* state) {
     sim_free(ctx);
     SimState* s = new SimState();
     ctx->sim = s;
@@ -543,6 +625,7 @@ int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p) {
     mt[0] = p->seed;
     for (int i = 1; i < kMtN; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
     mt[kMtN] = kMtN;
+    if (state) mt.assign(state, state + kMtN + 1);
     if (!(s->mt = dev_copy(mt.data(), mt.size(), s->owned))) return fail();
     SIM_ALLOC(s->words[0], (size_t)s->W + s->L);
     SIM_ALLOC(s->words[1], (size_t)s->W + s->L);
@@ -578,10 +661,101 @@ int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p) {
     for (cudaEvent_t& x : s->ph_ev) RB_CUDA(cudaEventCreate(&x));
     RB_CUDA(cudaEventRecord(s->used_ev[0], ctx->stream));  // the buffers are free; counts are zeroed first
     RB_CUDA(cudaEventRecord(s->used_ev[1], ctx->stream));
-    if (int rc = sim_enqueue_gen(s, 0)) return rc;
+    return 0;
+}
+
+}  // namespace
+
+int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p) {
+    if (int rc = sim_setup(ctx, p, nullptr)) return rc;
+    if (int rc = sim_enqueue_gen(ctx->sim, 0)) return rc;
     ctx->launches += 1;
     return 0;
 }
+
+namespace {
+
+constexpr int kTb = 256;
+
+// 2. + the doubling tables of step 3 for the window in `words`, from start position `first` on
+void sim_lengths(SimState* s, cudaStream_t st, const uint32_t* words, uint32_t first) {
+    const uint32_t W = s->W, span = W - first;
+    const unsigned gw = (W + 1 + kTb - 1) / kTb, gs_ = (span + 1 + kTb - 1) / kTb;
+    if (s->exact_body) sim_len_kernel<kWalk><<<gw, kTb, 0, st>>>(s->t, words, first, W, s->len, s->jump[0]);
+    else sim_len_kernel<kCount><<<gw, kTb, 0, st>>>(s->t, words, first, W, s->len, s->jump[0]);
+    for (uint32_t k = 1; k <= s->K; ++k) sim_double_kernel<<<gs_, kTb, 0, st>>>(s->jump[k - 1], s->jump[k], first, W);
+}
+
+// 3. the chain of attempts from the entry point `first`, keeping at most `need` successes: io = the exit (in this
+// window's frame), the successes and the failures.  Records ph_ev[1] and waits for the stream.
+int sim_resolve(SimState* s, cudaStream_t st, uint32_t first, uint64_t need, uint64_t io[3]) {
+    const uint32_t W = s->W, span = W - first;
+    const unsigned gs_ = (span + 1 + kTb - 1) / kTb;
+    RB_CUDA(cudaMemsetAsync(s->mark, 0, (size_t)W + 1, st));
+    RB_CUDA(cudaMemsetAsync(s->mark + first, 1, 1, st));
+    for (int k = (int)s->K; k >= 0; --k) sim_mark_kernel<<<gs_, kTb, 0, st>>>(s->jump[k], s->mark, first, W);
+    RB_CUDA(cub::DeviceSelect::Flagged(s->scan_tmp, s->scan_tmp_bytes, thrust::counting_iterator<uint32_t>(0),
+                                       s->mark, s->chain, s->n_chain, (int)W, st));
+    sim_okflag_kernel<<<gs_, kTb, 0, st>>>(s->chain, s->n_chain, s->len, s->cum);
+    RB_CUDA(cub::DeviceScan::InclusiveSum(s->scan_tmp, s->scan_tmp_bytes, s->cum, s->cum, (int)span, st));
+    sim_cut_kernel<<<gs_, kTb, 0, st>>>(s->chain, s->n_chain, s->cum, s->len, need, s->starts, s->io);
+    RB_CUDA(cudaMemcpyAsync(io, s->io, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    RB_CUDA(cudaEventRecord(s->ph_ev[1], st));
+    RB_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// 4. + 5. the n reads resolved in buffer b, numbered from rid0, as text in the host buffers of the next slot
+int sim_emit(rsem_b200_ctx* ctx, SimState* s, int b, uint32_t n, uint64_t rid0, const char* text[2], uint64_t bytes[2]) {
+    cudaStream_t st = ctx->stream;
+    const uint32_t* words = s->words[b];
+    const bool paired = s->t.type >= 2;
+    const int nm = paired ? 2 : 1;
+    const unsigned gb = (n + kTb - 1) / kTb;
+    RB_CUDA(cudaEventRecord(s->ph_ev[0], st));
+    if (s->exact_body)
+        sim_head_kernel<kWalk><<<gb, kTb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1]);
+    else
+        sim_head_kernel<kCount><<<gb, kTb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1]);
+    uint64_t tot[2] = {0, 0};
+    for (int m = 0; m < nm; ++m) {
+        RB_CUDA(cudaMemsetAsync(s->bytes[m] + n, 0, sizeof(uint64_t), st));
+        RB_CUDA(cub::DeviceScan::ExclusiveSum(s->scan_tmp, s->scan_tmp_bytes, s->bytes[m], s->bytes[m], (int)n + 1, st));
+        RB_CUDA(cudaMemcpyAsync(&tot[m], s->bytes[m] + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    }
+    RB_CUDA(cudaStreamSynchronize(st));
+    const size_t need = std::max(tot[0], tot[1]);
+    if (need > s->text_cap) {
+        RB_CUDA(cudaStreamSynchronize(st));
+        cudaFree(s->text_d[0]);
+        cudaFree(s->text_d[1]);
+        s->text_d[0] = s->text_d[1] = nullptr;
+        s->text_cap = need + need / 4;
+        RB_CUDA(cudaMalloc(&s->text_d[0], s->text_cap));
+        if (paired) RB_CUDA(cudaMalloc(&s->text_d[1], s->text_cap));
+    }
+    sim_write_kernel<<<gb, kTb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1],
+                                         s->text_d[0], s->text_d[1], s->counts);
+    RB_CUDA(cudaEventRecord(s->ph_ev[2], st));
+    RB_CUDA(cudaEventRecord(s->used_ev[b], st));
+    ctx->launches += 2 + nm;
+    auto& th = s->text_h[s->slot];
+    s->slot ^= 1;
+    for (int m = 0; m < nm; ++m) {
+        th[m].resize(tot[m]);
+        RB_CUDA(cudaMemcpyAsync(th[m].data(), s->text_d[m], tot[m], cudaMemcpyDeviceToHost, st));
+        text[m] = th[m].data();
+        bytes[m] = tot[m];
+    }
+    RB_CUDA(cudaEventRecord(s->ph_ev[3], st));
+    RB_CUDA(cudaStreamSynchronize(st));
+    RB_CUDA(cudaGetLastError());
+    s->stats.reads_ms += elapsed(s->ph_ev[0], s->ph_ev[2]);
+    s->stats.copy_ms += elapsed(s->ph_ev[2], s->ph_ev[3]);
+    return 0;
+}
+
+}  // namespace
 
 int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {
     SimState* s = ctx->sim;
@@ -590,35 +764,18 @@ int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_
     *n_reads = 0;
     bytes[0] = bytes[1] = 0;
     text[0] = text[1] = nullptr;
-    const bool paired = s->t.type >= 2;
-    const int nm = paired ? 2 : 1;
-    const int tb = 256;
     while (*n_reads == 0 && s->done < s->N) {
         const uint32_t W = s->W;
         const int b = (int)(s->window & 1);
         // the next window's words are generated while this one is resolved and read
         if (int rc = sim_enqueue_gen(s, s->window + 1)) return rc;
         RB_CUDA(cudaStreamWaitEvent(st, s->gen_ev[b][1], 0));
-        const uint32_t* words = s->words[b];
 
         RB_CUDA(cudaEventRecord(s->ph_ev[0], st));
-        const uint32_t first = s->entry, span = W - first;
-        const unsigned gw = (W + 1 + tb - 1) / tb, gs_ = (span + 1 + tb - 1) / tb;
-        if (s->exact_body) sim_len_kernel<kWalk><<<gw, tb, 0, st>>>(s->t, words, first, W, s->len, s->jump[0]);
-        else sim_len_kernel<kCount><<<gw, tb, 0, st>>>(s->t, words, first, W, s->len, s->jump[0]);
-        for (uint32_t k = 1; k <= s->K; ++k) sim_double_kernel<<<gs_, tb, 0, st>>>(s->jump[k - 1], s->jump[k], first, W);
-        RB_CUDA(cudaMemsetAsync(s->mark, 0, (size_t)W + 1, st));
-        RB_CUDA(cudaMemsetAsync(s->mark + first, 1, 1, st));
-        for (int k = (int)s->K; k >= 0; --k) sim_mark_kernel<<<gs_, tb, 0, st>>>(s->jump[k], s->mark, first, W);
-        RB_CUDA(cub::DeviceSelect::Flagged(s->scan_tmp, s->scan_tmp_bytes, thrust::counting_iterator<uint32_t>(0),
-                                           s->mark, s->chain, s->n_chain, (int)W, st));
-        sim_okflag_kernel<<<gs_, tb, 0, st>>>(s->chain, s->n_chain, s->len, s->cum);
-        RB_CUDA(cub::DeviceScan::InclusiveSum(s->scan_tmp, s->scan_tmp_bytes, s->cum, s->cum, (int)span, st));
-        sim_cut_kernel<<<gs_, tb, 0, st>>>(s->chain, s->n_chain, s->cum, s->len, s->N - s->done, s->starts, s->io);
+        const uint32_t first = s->entry;
+        sim_lengths(s, st, s->words[b], first);
         uint64_t io[3];
-        RB_CUDA(cudaMemcpyAsync(io, s->io, sizeof io, cudaMemcpyDeviceToHost, st));
-        RB_CUDA(cudaEventRecord(s->ph_ev[1], st));
-        RB_CUDA(cudaStreamSynchronize(st));
+        if (int rc = sim_resolve(s, st, first, s->N - s->done, io)) return rc;
         ctx->launches += 5 + 2 * s->K + 2;
         s->entry = (uint32_t)(io[0] - W);  // < L: an attempt starting inside the window ends before W + L
         s->resim += io[2];
@@ -631,48 +788,7 @@ int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_
             RB_CUDA(cudaEventRecord(s->used_ev[b], st));
             continue;
         }
-        const uint64_t rid0 = s->done;
-        const unsigned gb = (n + tb - 1) / tb;
-        RB_CUDA(cudaEventRecord(s->ph_ev[0], st));
-        if (s->exact_body)
-            sim_head_kernel<kWalk><<<gb, tb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1]);
-        else
-            sim_head_kernel<kCount><<<gb, tb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1]);
-        uint64_t tot[2] = {0, 0};
-        for (int m = 0; m < nm; ++m) {
-            RB_CUDA(cudaMemsetAsync(s->bytes[m] + n, 0, sizeof(uint64_t), st));
-            RB_CUDA(cub::DeviceScan::ExclusiveSum(s->scan_tmp, s->scan_tmp_bytes, s->bytes[m], s->bytes[m], (int)n + 1, st));
-            RB_CUDA(cudaMemcpyAsync(&tot[m], s->bytes[m] + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-        }
-        RB_CUDA(cudaStreamSynchronize(st));
-        const size_t need = std::max(tot[0], tot[1]);
-        if (need > s->text_cap) {
-            RB_CUDA(cudaStreamSynchronize(st));
-            cudaFree(s->text_d[0]);
-            cudaFree(s->text_d[1]);
-            s->text_d[0] = s->text_d[1] = nullptr;
-            s->text_cap = need + need / 4;
-            RB_CUDA(cudaMalloc(&s->text_d[0], s->text_cap));
-            if (paired) RB_CUDA(cudaMalloc(&s->text_d[1], s->text_cap));
-        }
-        sim_write_kernel<<<gb, tb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1],
-                                            s->text_d[0], s->text_d[1], s->counts);
-        RB_CUDA(cudaEventRecord(s->ph_ev[2], st));
-        RB_CUDA(cudaEventRecord(s->used_ev[b], st));
-        ctx->launches += 2 + nm;
-        auto& th = s->text_h[s->slot];
-        s->slot ^= 1;
-        for (int m = 0; m < nm; ++m) {
-            th[m].resize(tot[m]);
-            RB_CUDA(cudaMemcpyAsync(th[m].data(), s->text_d[m], tot[m], cudaMemcpyDeviceToHost, st));
-            text[m] = th[m].data();
-            bytes[m] = tot[m];
-        }
-        RB_CUDA(cudaEventRecord(s->ph_ev[3], st));
-        RB_CUDA(cudaStreamSynchronize(st));
-        RB_CUDA(cudaGetLastError());
-        s->stats.reads_ms += elapsed(s->ph_ev[0], s->ph_ev[2]);
-        s->stats.copy_ms += elapsed(s->ph_ev[2], s->ph_ev[3]);
+        if (int rc = sim_emit(ctx, s, b, n, s->done, text, bytes)) return rc;
         s->stats.windows = s->window;
         s->done += n;
         *n_reads = n;
@@ -687,6 +803,205 @@ int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_s
     if (resim) *resim = s->resim;
     if (stats) { s->stats.windows = s->window; *stats = s->stats; }
     sim_free(ctx);
+    return 0;
+}
+
+// ---- several contexts ------------------------------------------------------------------------------------------------
+// Window w (words [w W, (w + 1) W + L)) belongs to context w mod G.  A context generates its window's W + L words with
+// sim_mt_kernel and then jumps its generator by (G - 1) W - L to the start of its next window (>= 0 as W >= L), on its
+// generator stream.  The attempt lengths and doubling tables do not depend on the entry point, so every context works
+// them out for its window as soon as the words are there (from start position 0); only the chain from the entry point
+// (sim_resolve) runs window after window, the exit of one window handed by the host to the context of the next.
+namespace {
+
+// boost's index after pos draws from the seeded state
+uint32_t mt_index_at(uint64_t pos) { return pos == 0 ? kMtN : (uint32_t)(pos - (uint64_t)kMtN * ((pos - 1) / kMtN)); }
+
+int sim_enqueue_gen_jump(rsem_b200_ctx* ctx, SimState* s, uint64_t lw) {
+    const int b = (int)(lw & 1);
+    cudaStream_t gs = s->gen_stream;
+    const uint64_t n = (uint64_t)s->W + s->L, J = (uint64_t)(s->G - 1) * s->W - s->L;
+    RB_CUDA(cudaStreamWaitEvent(gs, s->used_ev[b], 0));  // window lw - 2 of this context is done with this buffer
+    RB_CUDA(cudaEventRecord(s->gen_ev[b][0], gs));
+    sim_mt_kernel<<<1, kMtN, 0, gs>>>(s->mt, s->words[b], n);
+    RB_CUDA(cudaEventRecord(s->jump_ev[b], gs));
+    const MtJumpPlan plan = mt_jump_plan(mt_index_at(s->gen_pos + n), J);
+    if (plan.blocks) {
+        const int v = (int)(plan.blocks - s->step_blocks);  // 0 or 1: the index before the jump lies in [1, 624]
+        sim_mt_jump_conv_kernel<<<s->step_nb[v], kMtN, 0, gs>>>(s->mt, s->step_poly[v], s->jump_conv);
+        sim_mt_jump_horner_kernel<<<1, kMtN, 0, gs>>>(s->mt, s->jump_conv, s->step_nb[v], plan.idx);
+        ctx->launches += 3;
+    } else {
+        sim_mt_jump_horner_kernel<<<1, kMtN, 0, gs>>>(s->mt, nullptr, 0, plan.idx);
+        ctx->launches += 2;
+    }
+    s->gen_pos += n + J;
+    RB_CUDA(cudaEventRecord(s->gen_ev[b][1], gs));
+    return 0;
+}
+
+int sim_enqueue_prep(rsem_b200_ctx* ctx, SimState* s, uint64_t lw) {
+    const int b = (int)(lw & 1);
+    RB_CUDA(cudaStreamWaitEvent(ctx->stream, s->gen_ev[b][1], 0));
+    RB_CUDA(cudaEventRecord(s->prep_ev[b][0], ctx->stream));
+    sim_lengths(s, ctx->stream, s->words[b], 0);
+    RB_CUDA(cudaEventRecord(s->prep_ev[b][1], ctx->stream));
+    ctx->launches += 1 + s->K;
+    return 0;
+}
+
+void free_all(const std::vector<rsem_b200_ctx*>& ctxs) {
+    for (rsem_b200_ctx* c : ctxs) {
+        cudaSetDevice(c->device);
+        sim_free(c);
+    }
+}
+
+double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+}  // namespace
+
+int sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_params* p, rsem_b200_sim_multi** out) {
+    auto m = std::make_unique<rsem_b200_sim_multi>();
+    m->ctx.assign(ctxs, ctxs + n);
+    m->N = p->N;
+    std::vector<uint32_t> seeded(kMtN + 1), state(kMtN + 1);  // boost::mt19937(seed)
+    seeded[0] = p->seed;
+    for (int i = 1; i < kMtN; ++i) seeded[i] = 1812433253u * (seeded[i - 1] ^ (seeded[i - 1] >> 30)) + (uint32_t)i;
+    seeded[kMtN] = kMtN;
+    // the jump between a context's windows moves its array step_blocks or step_blocks + 1 twists; g = x^(624 (k - 1))
+    uint64_t step_blocks = 0;
+    std::vector<uint32_t> step_h[2];
+    int step_nb[2] = {0, 0};
+    for (int g = 0; g < n; ++g) {
+        rsem_b200_ctx* ctx = ctxs[g];
+        auto fail = [&](int rc) { free_all(m->ctx); return rc; };
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
+        if (int rc = sim_setup(ctx, p, nullptr)) return fail(rc);
+        SimState* s = ctx->sim;
+        if (g == 0) {
+            const uint64_t J = (uint64_t)(n - 1) * s->W - s->L;
+            step_blocks = J / kMtN;
+            for (int v = 0; v < 2; ++v) {
+                if (step_blocks + v == 0) continue;
+                std::vector<uint64_t> poly(kMtPolyWords);
+                if (!mt_jump_poly((step_blocks + v - 1) * kMtN, poly.data())) {
+                    set_error("sim_begin_devices: mt19937 characteristic polynomial not found");
+                    return fail(RSEM_B200_ERR_CUDA);
+                }
+                step_h[v].resize(kMtJumpBlocks * kMtBlockWords);
+                step_nb[v] = mt_jump_blocks(poly.data(), step_h[v].data());
+            }
+        }
+        s->G = n;
+        s->gen_pos = (uint64_t)g * s->W;
+        s->step_blocks = step_blocks;
+        if (g > 0) {
+            if (int rc = rsem_b200_mt19937_jump(seeded.data(), s->gen_pos, state.data())) return fail(rc);
+            if (cudaMemcpy(s->mt, state.data(), state.size() * sizeof(uint32_t), cudaMemcpyHostToDevice) != cudaSuccess)
+                return fail(cuda_fail(cudaGetLastError(), "cudaMemcpy", __FILE__, __LINE__));
+        }
+        for (int v = 0; v < 2; ++v) {
+            s->step_nb[v] = step_nb[v];
+            if (step_h[v].empty()) continue;
+            if (!(s->step_poly[v] = dev_copy(step_h[v].data(), step_h[v].size(), s->owned))) {
+                set_error("sim_begin_devices: cudaMalloc / cudaMemcpy failed");
+                return fail(RSEM_B200_ERR_CUDA);
+            }
+        }
+        auto setup = [&]() -> int {
+            SIM_ALLOC(s->jump_conv, (size_t)kMtJumpBlocks * kMtN);
+            for (cudaEvent_t& x : s->jump_ev) RB_CUDA(cudaEventCreate(&x));
+            for (auto& e : s->prep_ev) for (cudaEvent_t& x : e) RB_CUDA(cudaEventCreate(&x));
+            if (int rc = sim_enqueue_gen_jump(ctx, s, 0)) return rc;
+            return sim_enqueue_prep(ctx, s, 0);
+        };
+        if (int rc = setup()) return fail(rc);
+    }
+    *out = m.release();
+    return 0;
+}
+
+int sim_next_devices(rsem_b200_sim_multi* m, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {
+    *n_reads = 0;
+    bytes[0] = bytes[1] = 0;
+    text[0] = text[1] = nullptr;
+    const size_t G = m->ctx.size();
+    while (*n_reads == 0 && m->done < m->N) {
+        rsem_b200_ctx* ctx = m->ctx[m->window % G];
+        RB_CUDA(cudaSetDevice(ctx->device));
+        SimState* s = ctx->sim;
+        RB_ARG(s, "sim_begin_devices must be called first");
+        cudaStream_t st = ctx->stream;
+        const uint64_t lw = s->window;
+        const int b = (int)(lw & 1);
+        // this context's next window is generated while this one is resolved and read
+        if (int rc = sim_enqueue_gen_jump(ctx, s, lw + 1)) return rc;
+        RB_CUDA(cudaEventRecord(s->ph_ev[0], st));
+        const double t0 = now_ms();
+        uint64_t io[3];
+        if (int rc = sim_resolve(s, st, m->entry, m->N - m->done, io)) return rc;
+        m->handoff_ms += now_ms() - t0;
+        ctx->launches += 5 + s->K;
+        m->entry = (uint32_t)(io[0] - s->W);
+        s->resim += io[2];
+        const uint32_t n = (uint32_t)io[1];
+        s->stats.generate_ms += elapsed(s->gen_ev[b][0], s->jump_ev[b]);
+        s->jump_ms += elapsed(s->jump_ev[b], s->gen_ev[b][1]);
+        s->stats.resolve_ms += elapsed(s->prep_ev[b][0], s->prep_ev[b][1]) + elapsed(s->ph_ev[0], s->ph_ev[1]);
+        s->stats.words += (uint64_t)s->W + s->L;
+        s->stats.windows = ++s->window;
+        ++m->window;
+        if (n == 0) {
+            RB_CUDA(cudaEventRecord(s->used_ev[b], st));
+        } else {
+            if (int rc = sim_emit(ctx, s, b, n, m->done, text, bytes)) return rc;
+            m->done += n;
+            *n_reads = n;
+        }
+        if (int rc = sim_enqueue_prep(ctx, s, lw + 1)) return rc;
+    }
+    return 0;
+}
+
+int sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rsem_b200_sim_devices_stats* stats,
+                    rsem_b200_sim_stats* per_device) {
+    std::unique_ptr<rsem_b200_sim_multi> own(m);
+    rsem_b200_sim_devices_stats sum{};
+    sum.handoff_ms = m->handoff_ms;
+    uint64_t r_sum = 0;
+    std::vector<double> c;
+    for (size_t g = 0; g < m->ctx.size(); ++g) {
+        rsem_b200_ctx* ctx = m->ctx[g];
+        RB_CUDA(cudaSetDevice(ctx->device));
+        SimState* s = ctx->sim;
+        if (!s) {
+            free_all(m->ctx);
+            RB_ARG(false, "sim_begin_devices must be called first");
+        }
+        if (counts && c.empty()) c.assign((size_t)s->t.M + 1, 0.0);
+        const double jump_ms = s->jump_ms;
+        std::vector<double> cg(c.size());
+        uint64_t r = 0;
+        rsem_b200_sim_stats st{};
+        if (int rc = sim_end(ctx, counts ? cg.data() : nullptr, &r, &st)) {
+            free_all(m->ctx);
+            return rc;
+        }
+        for (size_t i = 0; i < c.size(); ++i) c[i] += cg[i];  // integers: any order gives the same sums
+        r_sum += r;
+        sum.jump_ms += jump_ms;
+        sum.sum.generate_ms += st.generate_ms;
+        sum.sum.resolve_ms += st.resolve_ms;
+        sum.sum.reads_ms += st.reads_ms;
+        sum.sum.copy_ms += st.copy_ms;
+        sum.sum.words += st.words;
+        sum.sum.windows += st.windows;
+        if (per_device) per_device[g] = st;
+    }
+    if (counts) std::copy(c.begin(), c.end(), counts);
+    if (resim) *resim = r_sum;
+    if (stats) *stats = sum;
     return 0;
 }
 

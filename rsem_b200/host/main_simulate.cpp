@@ -9,6 +9,8 @@
 //
 // RSEM_B200_SIM_WINDOW=<words> sets the device's stream window (tests use small windows to cross many window bounds);
 // RSEM_B200_TIMING=1 prints the device time of each phase and the time spent waiting for file writes to stderr.
+// RSEM_B200_DEVICES=a,b,... with more than one entry spreads the stream's windows over those devices (an entry may
+// repeat: several contexts on one card), with the same output; otherwise RSEM_B200_DEVICE picks the one device.
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -195,10 +197,19 @@ int main(int argc, char* argv[]) {
     auto now = []() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     double t_dev = 0, t_io = 0;
 
+    const std::vector<int> devices = gpu_devices();
     rsem_b200_ctx* ctx = nullptr;
-    const char* dev = getenv("RSEM_B200_DEVICE");
-    check_rc(rsem_b200_ctx_create(dev ? atoi(dev) : 0, &ctx), "ctx_create");
-    check_rc(rsem_b200_sim_begin(ctx, &p), "sim_begin");
+    LaneContexts lanes;
+    rsem_b200_sim_multi* multi = nullptr;
+    if (devices.size() > 1) {
+        lanes = open_lanes(devices);
+        if (!lanes.err.empty()) die(lanes.err);
+        check_rc(rsem_b200_sim_begin_devices(lanes.ctx.data(), (int)lanes.ctx.size(), &p, &multi), "sim_begin_devices");
+    } else {
+        const char* dev = getenv("RSEM_B200_DEVICE");
+        check_rc(rsem_b200_ctx_create(dev ? atoi(dev) : 0, &ctx), "ctx_create");
+        check_rc(rsem_b200_sim_begin(ctx, &p), "sim_begin");
+    }
     // the read text of one chunk is written on a second thread while the device produces the next chunk (the library
     // keeps a chunk's buffers until the second following sim_next)
     uint64_t done = 0;
@@ -210,7 +221,8 @@ int main(int argc, char* argv[]) {
         const char* text[2];
         uint64_t bytes[2], n = 0;
         double t0 = now();
-        check_rc(rsem_b200_sim_next(ctx, text, bytes, &n), "sim_next");
+        if (multi) check_rc(rsem_b200_sim_next_devices(multi, text, bytes, &n), "sim_next_devices");
+        else check_rc(rsem_b200_sim_next(ctx, text, bytes, &n), "sim_next");
         t_dev += now() - t0;
         t0 = now();
         finish_write();
@@ -233,8 +245,16 @@ int main(int argc, char* argv[]) {
     std::vector<double> counts((size_t)M + 1, 0.0);
     uint64_t resim = 0;
     rsem_b200_sim_stats st;
-    check_rc(rsem_b200_sim_end(ctx, counts.data(), &resim, &st), "sim_end");
-    rsem_b200_ctx_destroy(ctx);
+    rsem_b200_sim_devices_stats dst{};
+    std::vector<rsem_b200_sim_stats> per(lanes.ctx.size());
+    if (multi) {
+        check_rc(rsem_b200_sim_end_devices(multi, counts.data(), &resim, &dst, per.data()), "sim_end_devices");
+        st = dst.sum;
+        for (rsem_b200_ctx* c : lanes.ctx) rsem_b200_ctx_destroy(c);
+    } else {
+        check_rc(rsem_b200_sim_end(ctx, counts.data(), &resim, &st), "sim_end");
+        rsem_b200_ctx_destroy(ctx);
+    }
     printf("Total number of resimulation is %llu\n", (unsigned long long)resim);
     fflush(stdout);
 
@@ -252,5 +272,15 @@ int main(int argc, char* argv[]) {
                 (unsigned long long)done, t_dev, t_io, st.generate_ms / 1e3, (unsigned long long)st.words,
                 st.generate_ms > 0 ? st.words / (st.generate_ms / 1e3) : 0.0, st.resolve_ms / 1e3, st.reads_ms / 1e3,
                 st.copy_ms / 1e3, (unsigned long long)st.windows);
+    if (timing && multi) {
+        fprintf(stderr, "rsem-simulate-reads timing: %zu devices (times summed over them): mt19937 jumps %.3f s "
+                "(overlapped), waiting for each window's entry point %.3f s\n", per.size(), dst.jump_ms / 1e3,
+                dst.handoff_ms / 1e3);
+        for (size_t g = 0; g < per.size(); ++g)
+            fprintf(stderr, "rsem-simulate-reads timing: device %d (entry %zu): stream generation %.3f s (%llu words), "
+                    "boundary resolution %.3f s, read generation + formatting %.3f s, copy to host %.3f s, windows %llu\n",
+                    devices[g], g, per[g].generate_ms / 1e3, (unsigned long long)per[g].words, per[g].resolve_ms / 1e3,
+                    per[g].reads_ms / 1e3, per[g].copy_ms / 1e3, (unsigned long long)per[g].windows);
+    }
     return 0;
 }
