@@ -7,9 +7,10 @@
 // same theta values and add to the same counts, so
 //
 //   * at upload the rows are sorted by (degree, hash of the id list) and verified pairwise -> classes;
-//   * a class is cut into SEGMENTS of <= R rows; a lane group owns a segment: it loads the ids and theta ONCE,
-//     walks the segment's rows keeping the normalised weights in per-lane accumulators and issues ONE reduction per
-//     transcript and segment (R x fewer gathers and reductions; singletons degrade to the row kernel's cost);
+//   * a class is cut into SEGMENTS of seg_rows(d, n) rows (as few as a batch allows); a lane group owns a segment: it
+//     loads the ids and theta ONCE, walks the segment's rows keeping the normalised weights in per-lane accumulators
+//     and issues ONE reduction per transcript and segment (rows-per-segment x fewer gathers and reductions;
+//     singletons degrade to the row kernel's cost);
 //   * 32 / G segments of equal (rows, degree) form a BATCH = the unit a warp claims; a batch's conprb / ncpv values
 //     are stored interleaved (value (segment gi, row r, column c) at (r d + c) nsb + gi) so that every warp-wide
 //     shared-memory load reads 32 consecutive doubles (no bank conflicts), with no padding in HBM;
@@ -64,6 +65,25 @@ __host__ __device__ __forceinline__ unsigned rows_cap(unsigned d, unsigned R) {
     const unsigned P = 32u / group_of_deg(d);
     const unsigned c = kMaxBatchVals / (P * (d + 1u));
     return c < 1u ? 1u : (c < R ? c : R);
+}
+
+// Rows per segment of a class of n rows and degree d (the default cut; RSEM_B200_CLASS_ROWS=R cuts every class into
+// rows_cap(d, R) instead).  Each segment pays one id load + theta gather and one reduction per transcript, so a class
+// is cut as little as a batch (P = 32 / G segments) allows:
+//   * n >= 8 P: rows_cap(d, 8).  Such a class fills one-class batches, whose P lane groups gather the same theta in one
+//     instruction and whose fold reduces once per batch; longer segments would save nothing;
+//   * smaller classes: ceil(n / cap) segments of cap = max(rows_cap(d, 8), min(8 P - 1, kBatchValBudget / (P (d + 1))))
+//     rows, so that a batch of such segments holds up to kBatchValBudget values.  The max keeps every class at no more
+//     segments than the 8-row cut; for P = 1 (G = 32 and the kTailCfg rows) cap is rows_cap(d, 8).
+// Segments stay <= 255 rows (8 P - 1 <= 255), the width of the row fields of BatchDesc and key2.
+constexpr unsigned kBatchValBudget = 2048;
+__host__ __device__ __forceinline__ unsigned seg_rows(unsigned d, unsigned n) {
+    const unsigned P = 32u / group_of_deg(d);
+    const unsigned r8 = rows_cap(d, 8u);
+    if (n >= 8u * P) return r8;
+    const unsigned v = kBatchValBudget / (P * (d + 1u));
+    const unsigned c = v < 8u * P - 1u ? v : 8u * P - 1u;
+    return c > r8 ? c : r8;
 }
 
 // A segment is a RUN when its ids are first, first + 1, ..., first + d - 1 (a row over consecutive transcripts: the
@@ -191,12 +211,22 @@ struct MaxOp {
     __device__ __forceinline__ unsigned operator()(unsigned a, unsigned b) const { return a > b ? a : b; }
 };
 
+// csize[start of class] = rows of the class, written by the class's last row
+__global__ void cls_class_size_kernel(const unsigned* __restrict__ cstart, unsigned n_rows, unsigned* csize) {
+    const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n_rows) return;
+    if (p + 1u == n_rows || cstart[p + 1u] == p + 1u) csize[cstart[p]] = p + 1u - cstart[p];
+}
+
+// R > 0: segments of rows_cap(d, R) rows; R == 0: segments of seg_rows(d, class size) rows
 __global__ void cls_seg_flag_kernel(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ cstart,
-                                    unsigned n_rows, unsigned R, unsigned* flag) {
+                                    const unsigned* __restrict__ csize, unsigned n_rows, unsigned R, unsigned* flag) {
     const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n_rows) return;
     const unsigned d = (unsigned)(keys[p] >> 48);
-    flag[p] = ((p - cstart[p]) % rows_cap(d, R)) == 0u ? 1u : 0u;
+    const unsigned c = cstart[p];
+    const unsigned rows = R ? rows_cap(d, R) : seg_rows(d, csize[c]);
+    flag[p] = ((p - c) % rows) == 0u ? 1u : 0u;
 }
 
 __global__ void cls_seg_scatter_kernel(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ cstart,
@@ -492,22 +522,21 @@ __device__ __forceinline__ double fast_rcp(double x) {
     return r;
 }
 
-// U rows of a batch at once.  ROWS_OK: all U rows exist (main loop) - otherwise rows >= n_left are idle (remainder).
+// U rows of a batch at once.
 // TAIL: the rows have more than G * S = 128 columns (configuration kTailCfg); the rest are walked from shared memory.
-template <int G, int S, int U, bool ROWS_OK, bool TAIL>
-__device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsigned row_stride, unsigned n_left,
-                                           const double (&th)[S], const bool (&col_ok)[S], const unsigned (&coff)[S],
-                                           double (&acc)[S], unsigned g, unsigned w, unsigned nsb, unsigned d,
+template <int G, int S, int U, bool TAIL>
+__device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsigned row_stride, const double (&th)[S],
+                                           const bool (&col_ok)[S], const unsigned (&coff)[S], double (&acc)[S],
+                                           unsigned g, unsigned w, unsigned nsb, unsigned d,
                                            const int* __restrict__ bi, unsigned ids_stride, unsigned ids_gi, bool seg_ok,
                                            const double* __restrict__ theta, double* count, double& acc0) {
     double x[U][S], part[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-        const bool row_ok = ROWS_OK || (unsigned)u < n_left;
 #pragma unroll
         for (int q = 0; q < S; ++q) {
             double c = 0.0;  // idle lanes must not read: the bytes behind a batch are arbitrary (possibly NaN patterns)
-            if (col_ok[q] && row_ok) c = cr[u * row_stride + coff[q]];
+            if (col_ok[q]) c = cr[u * row_stride + coff[q]];
             x[u][q] = th[q] * c;
             if (x[u][q] < kEpsilon) x[u][q] = 0.0;
         }
@@ -522,11 +551,9 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
             const double thc = __ldg(theta + (c < d ? bi[c * ids_stride + ids_gi] : 0));
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-                if (ROWS_OK || (unsigned)u < n_left) {
-                    double f = thc * cr[u * row_stride + c * nsb];
-                    if (f < kEpsilon) f = 0.0;
-                    part[u] += f;
-                }
+                double f = thc * cr[u * row_stride + c * nsb];
+                if (f < kEpsilon) f = 0.0;
+                part[u] += f;
             }
         }
     }
@@ -534,10 +561,10 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
     for (int u = 0; u < U; ++u) part[u] = seg_sum<G>(part[u]);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-        const double inv = part[u] >= kEpsilon ? fast_rcp(part[u]) : 0.0;  // idle rows: part = 0 -> inv = 0
+        const double inv = part[u] >= kEpsilon ? fast_rcp(part[u]) : 0.0;
 #pragma unroll
         for (int q = 0; q < S; ++q) acc[q] += x[u][q] * inv;
-        if (TAIL && seg_ok && (ROWS_OK || (unsigned)u < n_left)) {
+        if (TAIL && seg_ok) {
             for (unsigned c = g + G * S; c < w; c += G) {
                 const int tt = c < d ? bi[c * ids_stride + ids_gi] : 0;
                 double f = __ldg(theta + tt) * cr[u * row_stride + c * nsb];
@@ -552,7 +579,8 @@ __device__ __forceinline__ void batch_rows(const double* __restrict__ cr, unsign
 
 // One batch: P = 32 / G segments of n rows x (d + 1) columns; lane = g * P + gi owns columns g, g + G, ... of segment
 // gi: ids and theta are loaded once, the rows are walked U at a time (instruction-level parallelism across the
-// load -> product -> row sum -> reciprocal chain), the normalised weights are summed per lane and leave as ONE
+// load -> product -> row sum -> reciprocal chain) and the last n % U two or one at a time, so that no pass walks rows
+// the segments do not have (many are shorter than U rows), the normalised weights are summed per lane and leave as ONE
 // reduction per transcript and segment.  The noise column's sum stays in the thread (count[0] is flushed per CTA).
 // run: the batch stores its segments' firsts, column c < d is transcript first + c.
 // PROF: ph[] takes the cycles from t0 (read by the caller before it loaded the batch's descriptor) to theta usable,
@@ -594,11 +622,16 @@ __device__ __forceinline__ double process_batch(const double* __restrict__ bv, c
     double acc0 = 0.0;
     unsigned r = 0;
     for (; r + U <= n; r += U)
-        batch_rows<G, S, U, true, TAIL>(con + (unsigned long long)r * row_stride, row_stride, U, th, col_ok, coff, acc, g, w, nsb, d,
-                                        bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
+        batch_rows<G, S, U, TAIL>(con + (unsigned long long)r * row_stride, row_stride, th, col_ok, coff, acc, g, w, nsb, d, bi,
+                                  ids_stride, ids_gi, seg_ok, theta, count, acc0);
+    if (U > 2 && r + 2 <= n) {
+        batch_rows<G, S, 2, TAIL>(con + (unsigned long long)r * row_stride, row_stride, th, col_ok, coff, acc, g, w, nsb, d, bi,
+                                  ids_stride, ids_gi, seg_ok, theta, count, acc0);
+        r += 2;
+    }
     if (U > 1 && r < n)
-        batch_rows<G, S, U, false, TAIL>(con + (unsigned long long)r * row_stride, row_stride, n - r, th, col_ok, coff, acc, g, w,
-                                         nsb, d, bi, ids_stride, ids_gi, seg_ok, theta, count, acc0);
+        batch_rows<G, S, 1, TAIL>(con + (unsigned long long)r * row_stride, row_stride, th, col_ok, coff, acc, g, w, nsb, d, bi,
+                                  ids_stride, ids_gi, seg_ok, theta, count, acc0);
     if (PROF) {
         const long long t1 = clk_after(acc[0]);
         ph[kPhRows] += t1 - t0;
@@ -891,8 +924,8 @@ int class_build(rsem_b200_ctx* ctx) {
     cudaStream_t st = ctx->stream;
     const unsigned long long* rp = reinterpret_cast<const unsigned long long*>(ctx->row_ptr);
     const int* sid_abs = ctx->sid_abs;
-    unsigned R = 8;
-    if (const char* e = getenv("RSEM_B200_CLASS_ROWS")) {  // tuning knob: rows per segment
+    unsigned R = 0;  // 0: seg_rows
+    if (const char* e = getenv("RSEM_B200_CLASS_ROWS")) {  // tuning knob: a fixed cut of rows per segment
         const int v = atoi(e);
         if (v >= 1 && v <= 255) R = (unsigned)v;
     }
@@ -953,7 +986,9 @@ int class_build(rsem_b200_ctx* ctx) {
     RB_CUDA(cudaGetLastError());
     need = tmp_bytes;
     RB_CUDA(cub::DeviceScan::InclusiveScan(tmp, need, a32, b32, MaxOp(), (long long)n_rows, st));  // b32 = class start
-    cls_seg_flag_kernel<<<blocks_for(n_rows, 256), 256, 0, st>>>(keys_s, b32, n_rows, R, a32);    // a32 = segment flag
+    cls_class_size_kernel<<<blocks_for(n_rows, 256), 256, 0, st>>>(b32, n_rows, c32);              // c32 = class size
+    RB_CUDA(cudaGetLastError());
+    cls_seg_flag_kernel<<<blocks_for(n_rows, 256), 256, 0, st>>>(keys_s, b32, c32, n_rows, R, a32);  // a32 = segment flag
     RB_CUDA(cudaGetLastError());
     need = tmp_bytes;
     RB_CUDA(cub::DeviceScan::InclusiveSum(tmp, need, a32, c32, (long long)n_rows, st));            // c32 = segment idx + 1
@@ -1118,7 +1153,7 @@ int class_build(rsem_b200_ctx* ctx) {
     L.R = R;
     L.built = true;
     L.vals_epoch = 0;
-    ctx->launches += 20;
+    ctx->launches += 21;
     return 0;
 }
 
@@ -1163,25 +1198,18 @@ int class_launch_estep(rsem_b200_ctx* ctx) {
         L.last_profiled = ctx->profiling;
         const unsigned grid = std::min<unsigned>((unsigned)ctx->sm_count, a.n_tiles);
         L.last_grid = grid;
-        // 15 consumer warps x 2 rows in flight per lane (98 registers, no spills).  Without the tail code more warps
-        // fit and hide more of a batch's latency (ids -> theta gather -> values -> row sums); 18 warps are no faster.
-        // Measured on H100 80GB HBM3 at 700 W, ms per round, median of 3 alternating runs in one process:
-        //   consumer warps x rows:  11x2   11x3   11x4   14x2   14x3   14x4   15x2   15x3   15x4   18x2   18x3   18x4
-        //   C3                      3.505  3.460  3.446  3.389  3.396  3.410  3.389  3.394  3.397  3.387  3.483  3.697
-        //   C2                      0.373  0.373  0.376  0.371  0.372  0.374  0.372  0.372  0.374  0.370  0.371  0.405
-        //   C5                      8.167  8.292  8.589  7.952  8.044  8.294  7.813  7.977  8.187  7.818  7.895  8.302
-        // (18 x 3 and 18 x 4 spill; the sweep predates the evict_first priority of the copies, which took 15 x 2 at C3
-        // from 3.39 to 3.20 ms.)  The previous kernel, with the tail code in every configuration (11 x 2, 167
-        // registers), in a separate process on the same card: C3 3.519, C2 0.373, C5 8.579.
-        // Re-swept with evict_first and run batches (same card, one process per run, 3 alternating runs, ms per round):
-        //   consumer warps x rows:  14x2                 15x2                 18x2
-        //   C3                      3.039 3.040 3.036    3.028 3.041 3.029    3.030 3.031 3.032
-        //   C2                      0.357 0.356 0.352    0.353 0.360 0.351    0.356 0.353 0.354
-        //   C5                      7.561 7.562 7.540    7.428 7.421 7.398    7.216 7.213 7.202
-        // 18 warps tie at C3 and C2 and are 2.7 % faster at C5 (88 registers), but their profiling instantiation
-        // spills (16 bytes), so 15 stays: the profiled launch (tools/k2_anatomy.py) has to run the configuration
-        // that is timed, or its phase shares describe another kernel, and no instantiation may spill.
-        constexpr int W = 15, U = 2;
+        // 15 consumer warps x 3 rows in flight per lane (102 registers, 116 in the profiling build, no spills).  Swept
+        // with the default segment rule, on H100 80GB HBM3 at 700 W, ms per round, median of 2 runs in one process per
+        // workload, all configurations alternating:
+        //   consumer warps x rows:  14x2   14x3   14x4   15x2   15x3   15x4
+        //   C3                      2.916  2.891  2.885  2.903  2.887  2.899
+        //   C2                      0.332  0.328  0.329  0.330  0.328  0.327
+        //   C5                      7.309  7.331  7.341  7.200  7.217  7.291
+        // Longer segments give the rows in flight more to overlap; 15 x 3 is among the fastest at C3 and C2 and within
+        // 0.3 % of the fastest at C5.  18 warps are left out: every one of their profiling instantiations spills (16-180
+        // bytes), and the profiled launch (tools/k2_anatomy.py) has to run the configuration that is timed, or its
+        // phase shares describe another kernel.
+        constexpr int W = 15, U = 3;
         const size_t smem = sizeof(ClassSmem<W>);
         if (ctx->profiling) {
             RB_CUDA(raise_dyn_smem((const void*)estep_class_kernel<W, U, false, true>, smem));
