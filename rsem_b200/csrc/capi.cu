@@ -143,17 +143,7 @@ void free_refs(rsem_b200_ctx* c) {
 }
 
 void free_gibbs(rsem_b200_ctx* c) {
-    if (c->gibbs.row_ptr) cudaFree(c->gibbs.row_ptr);
-    if (c->gibbs.sid) cudaFree(c->gibbs.sid);
-    if (c->gibbs.conprb) cudaFree(c->gibbs.conprb);
-    if (c->gibbs.order) cudaFree(c->gibbs.order);
-    if (c->gibbs.p_off) cudaFree(c->gibbs.p_off);
-    if (c->gibbs.p_sid) cudaFree(c->gibbs.p_sid);
-    if (c->gibbs.p_con) cudaFree(c->gibbs.p_con);
-    if (c->gibbs.seg_start) cudaFree(c->gibbs.seg_start);
-    if (c->gibbs.seg_ntr) cudaFree(c->gibbs.seg_ntr);
-    if (c->gibbs.seg_tid_off) cudaFree(c->gibbs.seg_tid_off);
-    if (c->gibbs.comp_tids) cudaFree(c->gibbs.comp_tids);
+    if (c->gibbs.block) cudaFree(c->gibbs.block);
     c->gibbs = DevGibbs{};
 }
 
@@ -729,19 +719,7 @@ int rsem_b200_gibbs_upload(rsem_b200_ctx* c, uint64_t N1, uint64_t E, int32_t M,
     RB_ARG(row_ptr[0] == 0 && row_ptr[N1] == E, "row_ptr must start at 0 and end at E");
     RB_CUDA(cudaSetDevice(c->device));
     free_gibbs(c);
-    RB_CUDA(cudaMalloc(&c->gibbs.row_ptr, (N1 + 1) * sizeof(uint64_t)));
-    RB_CUDA(cudaMalloc(&c->gibbs.sid, (E + 4) * sizeof(int32_t)));
-    RB_CUDA(cudaMalloc(&c->gibbs.conprb, (E + 4) * sizeof(double)));
-    RB_CUDA(cudaMemcpyAsync(c->gibbs.row_ptr, row_ptr, (N1 + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(c->gibbs.sid, sid, E * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(c->gibbs.conprb, conprb, E * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
-    c->gibbs.N1 = N1;
-    c->gibbs.E = E;
-    c->gibbs.M = M;
-    if (int rc = gibbs_prepare(c, row_ptr, sid)) return rc;
-    c->gibbs.ready = true;
-    return 0;
+    return gibbs_upload(c, N1, E, M, row_ptr, sid, conprb);
 }
 
 int rsem_b200_gibbs_upload_from(rsem_b200_ctx* dst, const rsem_b200_ctx* src) {
@@ -760,41 +738,23 @@ int rsem_b200_gibbs_upload_from(rsem_b200_ctx* dst, const rsem_b200_ctx* src) {
         }
     }
     const DevGibbs& s = src->gibbs;
-    DevGibbs& d = dst->gibbs;
-    d.N1 = s.N1; d.E = s.E; d.M = s.M;
-    d.n_comp_tids = s.n_comp_tids; d.n_segs = s.n_segs; d.max_len = s.max_len; d.empty_row = s.empty_row;
-    // same allocation sizes as gibbs_upload / gibbs_prepare; the padding past the data is never copied there either
-    auto copy = [&](auto** to, const auto* from, size_t alloc, size_t n) -> int {
-        if (!from) return 0;
-        RB_CUDA(cudaMalloc(to, alloc * sizeof(**to)));
-        if (n) RB_CUDA(cudaMemcpyPeerAsync(*to, dst->device, from, src->device, n * sizeof(**to), dst->stream));
-        return 0;
-    };
-    int rc = 0;
-    const size_t n_segs = (size_t)s.n_segs;
-    if (!rc) rc = copy(&d.row_ptr, s.row_ptr, s.N1 + 1, s.N1 + 1);
-    if (!rc) rc = copy(&d.sid, s.sid, s.E + 4, s.E);
-    if (!rc) rc = copy(&d.conprb, s.conprb, s.E + 4, s.E);
-    if (!rc) rc = copy(&d.order, s.order, s.N1, s.N1);
-    if (!rc) rc = copy(&d.p_off, s.p_off, s.N1 + 1, s.N1 + 1);
-    if (!rc) rc = copy(&d.p_sid, s.p_sid, s.E + 16, s.E);
-    if (!rc) rc = copy(&d.p_con, s.p_con, s.E + 16, s.E);
-    if (!rc) rc = copy(&d.seg_start, s.seg_start, n_segs + 1, n_segs + 1);
-    if (!rc) rc = copy(&d.seg_ntr, s.seg_ntr, std::max<size_t>(n_segs, 1), n_segs);
-    if (!rc) rc = copy(&d.seg_tid_off, s.seg_tid_off, n_segs + 1, n_segs + 1);
-    if (!rc) rc = copy(&d.comp_tids, s.comp_tids, s.n_comp_tids, s.n_comp_tids);
-    if (!rc) {
-        const cudaError_t e = cudaStreamSynchronize(dst->stream);
-        if (e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    void* block = nullptr;
+    RB_CUDA(cudaMalloc(&block, s.bytes));
+    cudaError_t e = cudaMemcpyPeerAsync(block, dst->device, s.block, src->device, s.bytes, dst->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(dst->stream);
+    if (e != cudaSuccess) {
+        cudaFree(block);
+        return cuda_fail(e, "gibbs_upload_from: copy", __FILE__, __LINE__);
     }
-    if (rc) { free_gibbs(dst); return rc; }
-    d.ready = true;
+    dst->gibbs = s;
+    dst->gibbs.block = block;
+    dst->gibbs.v = gibbs_view(block, s.N1, s.E, s.M);
     return 0;
 }
 
 static int check_gibbs_run(const rsem_b200_ctx* c, const rsem_b200_gibbs_params* p) {
     RB_ARG(c && p, "NULL argument");
-    RB_ARG(c->gibbs.row_ptr, "gibbs_upload must be called first");
+    RB_ARG(c->gibbs.ready, "gibbs_upload must be called first");
     RB_ARG(p->M == c->gibbs.M, "M mismatch");
     RB_ARG(p->n_chains >= 1 && p->chain_samples && p->chain_seeds, "bad chain parameters");
     return 0;

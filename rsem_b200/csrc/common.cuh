@@ -98,22 +98,29 @@ struct DevRefs {
     uint32_t* mask_words = nullptr;
 };
 
+// typed pointers into DevGibbs::block (gibbs_view)
+struct GibbsView {
+    // component-parallel sampler (gibbs_kernels.cu): reads grouped by connected component
+    const int32_t* order = nullptr;      // N1 read ids: component by component (longest first), read order inside
+    const uint64_t* p_off = nullptr;     // rows re-laid in that slot order
+    const int32_t* p_sid = nullptr;
+    const double* p_con = nullptr;
+    const int32_t* seg_start = nullptr;  // n_segs + 1 offsets into `order`
+    const int32_t* seg_ntr = nullptr;    // transcripts per component; < 32: rows (p_sid) and assignments hold local ids
+    const int32_t* seg_tid_off = nullptr;
+    const int32_t* comp_tids = nullptr;  // sorted transcript ids of every component
+    // the rows as uploaded (serial kernel)
+    const uint64_t* row_ptr = nullptr;
+    const int32_t* sid = nullptr;
+    const double* conprb = nullptr;
+};
+
 struct DevGibbs {
     uint64_t N1 = 0, E = 0;
     int M = 0;
-    uint64_t* row_ptr = nullptr;
-    int32_t* sid = nullptr;
-    double* conprb = nullptr;
-    // component-parallel sampler (gibbs_kernels.cu): reads grouped by connected component
-    int32_t* order = nullptr;      // N1 read ids: component by component (longest first), read order inside
-    uint64_t* p_off = nullptr;     // rows re-laid in that slot order
-    int32_t* p_sid = nullptr;
-    double* p_con = nullptr;
-    int32_t* seg_start = nullptr;  // n_segs + 1 offsets into `order`
-    int32_t* seg_ntr = nullptr;    // transcripts per component; < 32: rows (p_sid) and assignments hold local ids
-    int32_t* seg_tid_off = nullptr;
-    int32_t* comp_tids = nullptr;  // sorted transcript ids of every component
-    size_t n_comp_tids = 0;        // entries of comp_tids
+    void* block = nullptr;         // one device allocation of `bytes` holding everything the view points to
+    size_t bytes = 0;
+    GibbsView v;
     int32_t n_segs = 0;
     uint32_t max_len = 0;
     bool empty_row = false;        // some read has no entry: gibbs_run refuses the matrix before any launch
@@ -354,9 +361,13 @@ int model_launch_update(rsem_b200_ctx* ctx);
 // gibbs_kernels.cu
 int gibbs_run(rsem_b200_ctx* ctx, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
               rsem_b200_gibbs_stats* stats);
-int gibbs_prepare(rsem_b200_ctx* ctx, const uint64_t* row_ptr, const int32_t* sid);
+// fills an empty ctx->gibbs: the rows and their component layout in one device block
+int gibbs_upload(rsem_b200_ctx* ctx, uint64_t N1, uint64_t E, int M, const uint64_t* row_ptr, const int32_t* sid,
+                 const double* conprb);
+// the view of a block that gibbs_upload filled for these sizes, wherever the block is
+GibbsView gibbs_view(void* block, uint64_t N1, uint64_t E, int M);
 // host side of the component-parallel sampler's layout (gibbs_kernels.cu): components, segments longest first, local
-// ids of register-resident components, rows in slot order.  gibbs_prepare and the Gibbs batch (K13) both build it.
+// ids of register-resident components, rows in slot order.  gibbs_upload and the Gibbs batch (K13) both build it.
 struct GibbsLayout {
     uint64_t N1 = 0;
     std::vector<int32_t> order;        // N1 read ids in slot order

@@ -14,8 +14,14 @@
 // the (count + alpha) * conprb products and the index count are spread over its 32 lanes, only the running sum is
 // serial) and gibbs_parallel_kernel (the product path: connected components of the read x transcript graph walked
 // concurrently by 16-lane groups, exact through a fixed-point iteration over the reads that change their noise
-// membership; see the block comment "Component-parallel EXACT sampler" below).  In both, the chain's CTA(s) also do the
-// O(M) per-sample work (count vector dump, theta -> polish -> TPM/FPKM, accumulation).
+// membership; see the block comment "Component-parallel EXACT sampler" below).  In both, a CTA of the chain also does the
+// O(M) per-sample work (keep_sample: count vector dump, theta -> polish -> TPM/FPKM, accumulation).
+//
+// Storage (gparts, scratch_parts): a sample is a layout part - the component layout, plus the uploaded rows the serial
+// kernel reads - and a run part - the inputs of a run, the chain states, slice totals and sums, the count vectors.  A
+// context holds its layout part in one block (DevGibbs; permute_rows_kernel re-lays conprb there) and each
+// rsem_b200_gibbs_run_chains call puts its run part and the per-chain scratch in another; a K13 batch sample holds both
+// parts in one block (conprb re-laid on the host) and its teams share the scratch.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -28,13 +34,23 @@ namespace rsem_b200 {
 namespace {
 
 constexpr int kGibbsThreads = 256;
+constexpr int kPThreads = 256;
+static_assert(kGibbsThreads == kPThreads, "the per-sample stage (keep_sample) runs in the CTAs of every Gibbs kernel");
 constexpr int kRowCap = 2048;  // cumulative-array slots in shared memory; longer rows use global scratch
 
-struct GibbsArgs {
-    unsigned long long N1;
-    const unsigned long long* row_ptr;
-    const int* sid;
-    const double* conprb;
+struct ChainSync {
+    unsigned count, gen;        // barrier among the chain's worker CTAs
+    unsigned u_ready;           // generator -> workers: uniforms of sweeps < u_ready are complete
+    unsigned sweeps_done;       // workers -> generator: sweeps < sweeps_done no longer need their uniform buffer
+    unsigned changed;           // some flip word differs between the pass's input and output sets
+    unsigned next_seg;          // next component to be claimed in the current pass
+    int err;                    // 3: a categorical draw fell off its cumulative array
+    unsigned passes;            // diagnostics: passes run over all sweeps
+    unsigned long long prof[4]; // clock64 totals of worker CTA 0: wait for uniforms, passes, barriers + bookkeeping, per-sample work
+};
+
+// What every Gibbs kernel reads about a run (run_args fills it from a run part).
+struct RunArgs {
     int M, burnin, gap, n_genes;
     const int* chain_samples;
     const unsigned* chain_seeds;
@@ -45,20 +61,35 @@ struct GibbsArgs {
     const double* eel;
     const double* mw;
     const int* gene_start;
-    // per-chain state / outputs
-    int* counts;          // n_chains * (M + 1)
-    int* z;               // n_chains * N1
-    double* scratch;      // n_chains * max_len (only when max_len > kRowCap)
-    unsigned max_len;
     int* count_vectors;   // total_samples * (M + 1)
     double* acc;          // n_chains * (4 * (M + 1) + n_genes): sum_c, sum_c2, sum_tpm, sum_fpkm, sum_gene_c2
-    double* theta_tmp;    // n_chains * 2 * (M + 1)  (theta / fpkm scratch)
-    int* err_flag;
+    double* theta_tmp;    // 2 * (M + 1) per chain slot (theta / fpkm scratch)
+    ChainSync* sync;      // n_chains
 };
+
+struct GibbsArgs : RunArgs {
+    unsigned long long N1;
+    const unsigned long long* row_ptr;
+    const int* sid;
+    const double* conprb;
+    int* counts;          // M + 1 per chain
+    int* z;               // N1 per chain
+    double* scratch;      // max_len per chain (read only when max_len > kRowCap)
+    unsigned max_len;
+};
+
+__device__ __forceinline__ int ld_cg(const int* p) { return __ldcg(p); }
+__device__ __forceinline__ void st_cg(int* p, int v) { __stcg(p, v); }
 
 struct MtState {
     unsigned mt[624];
 };
+
+// init_genrand (boost mt19937 seeding), by one thread
+__device__ __forceinline__ void mt_seed(unsigned* mt, unsigned seed) {
+    mt[0] = seed;
+    for (int k = 1; k < 624; ++k) mt[k] = 1812433253u * (mt[k - 1] ^ (mt[k - 1] >> 30)) + (unsigned)k;
+}
 
 __device__ __forceinline__ unsigned mt_twist(unsigned a, unsigned b, unsigned c) {
     const unsigned y = (a & 0x80000000u) | (b & 0x7fffffffu);
@@ -113,9 +144,57 @@ __device__ double block_sum(double v, double* sh) {
     return t;
 }
 
+// Gibbs.cpp:313-346 for kept sample `kept` of a chain, by one CTA (every thread calls): the count-vector row `cv`,
+// theta = (c + alpha) / totc (zero for omitted transcripts), polishTheta, TPM / FPKM and the five sums `acc`.  The counts
+// are read through L2: in K5 / K13 other CTAs of the chain wrote them.  tid, M1 and sh_red are the caller's: derived here
+// instead, they cost K5 and K13 more spills.
+__device__ __forceinline__ void keep_sample(const RunArgs& a, const int* counts, int* cv, double* acc, double* theta, int kept, int tid, int M1,
+                                            double* sh_red) {
+    double* fpkm = theta + M1;
+    double part = 0.0;
+    for (int i = tid; i < M1; i += kPThreads) {
+        const int c = ld_cg(counts + i);
+        cv[(size_t)kept * M1 + i] = c;
+        double th = c < 0 ? 0.0 : ((double)c + a.alpha[i]) / a.totc;
+        if (i > 0 && (a.mw[i] < kEpsilon || a.eel[i] < kEpsilon)) th = 0.0;
+        else th = th / a.mw[i];
+        theta[i] = th;
+        part += th;
+    }
+    const double tsum = block_sum(part, sh_red);
+    part = 0.0;
+    for (int i = tid; i < M1; i += kPThreads) {
+        const double th = theta[i] / tsum;
+        theta[i] = th;
+        if (i > 0 && a.eel[i] >= kEpsilon) part += th;
+    }
+    double denom = block_sum(part, sh_red);
+    if (denom < kEpsilon) denom = 1.0;
+    part = 0.0;
+    for (int i = tid; i < M1; i += kPThreads) {
+        const double f = (i > 0 && a.eel[i] >= kEpsilon) ? (theta[i] / denom) * 1e9 / a.eel[i] : 0.0;
+        fpkm[i] = f;
+        part += f;
+    }
+    double fsum = block_sum(part, sh_red);
+    if (fsum < kEpsilon) fsum = 1.0;
+    for (int i = tid; i < M1; i += kPThreads) {
+        const double c = (double)ld_cg(counts + i);
+        acc[i] += c;
+        acc[M1 + i] += c * c;
+        acc[2 * (size_t)M1 + i] += i > 0 ? fpkm[i] / fsum * 1e6 : 0.0;
+        acc[3 * (size_t)M1 + i] += fpkm[i];
+    }
+    for (int gi = tid; gi < a.n_genes; gi += kPThreads) {
+        double c = 0.0;
+        for (int j = a.gene_start[gi]; j < a.gene_start[gi + 1]; ++j) c += ld_cg(counts + j);
+        acc[4 * (size_t)M1 + gi] += c * c;
+    }
+}
+
 // one draw for read i by warp 0 (all 32 lanes call).  use_counts = false for the initial state.
 __device__ __forceinline__ void draw_read(const GibbsArgs& a, unsigned long long i, bool use_counts, int* counts, int* z,
-                                          double* s_arr, double* g_arr, MtState& mt, int& mt_idx, int lane) {
+                                          double* s_arr, double* g_arr, MtState& mt, int& mt_idx, int lane, int* err) {
     const unsigned long long fr = a.row_ptr[i], to = a.row_ptr[i + 1];
     const unsigned len = (unsigned)(to - fr);
     double* arr = len <= kRowCap ? s_arr : g_arr;
@@ -148,7 +227,7 @@ __device__ __forceinline__ void draw_read(const GibbsArgs& a, unsigned long long
     for (unsigned k = lane; k < len; k += 32) below += arr[k] <= prb;
     for (int o = 16; o > 0; o >>= 1) below += __shfl_xor_sync(0xffffffffu, below, o);
     if (below >= (int)len) {  // reference: assert(l < len), sampling.h:62
-        *a.err_flag = 3;
+        *err = 3;
         below = (int)len - 1;
     }
     __syncwarp();
@@ -168,72 +247,30 @@ __global__ void __launch_bounds__(kGibbsThreads) gibbs_chain_kernel(const GibbsA
     const int M1 = a.M + 1;
     int* counts = a.counts + (size_t)chain * M1;
     int* z = a.z + (size_t)chain * a.N1;
-    double* g_arr = a.scratch ? a.scratch + (size_t)chain * a.max_len : nullptr;
+    double* g_arr = a.scratch + (size_t)chain * a.max_len;
+    int* err = &a.sync[chain].err;
     double* acc = a.acc + (size_t)chain * (4 * (size_t)M1 + a.n_genes);
     double* theta = a.theta_tmp + (size_t)chain * 2 * M1;
-    double* fpkm = theta + M1;
     const int n_samples = a.chain_samples[chain];
     int* cv = a.count_vectors + a.chain_cv_offset[chain] * M1;
 
     for (int i = tid; i < M1; i += blockDim.x) counts[i] = a.init_counts[i] + (i == 0 ? (int)a.n0 : 0);
-    if (tid == 0) {  // init_genrand (boost mt19937 seeding)
-        mt.mt[0] = a.chain_seeds[chain];
-        for (int k = 1; k < 624; ++k) mt.mt[k] = 1812433253u * (mt.mt[k - 1] ^ (mt.mt[k - 1] >> 30)) + (unsigned)k;
-    }
+    if (tid == 0) mt_seed(mt.mt, a.chain_seeds[chain]);
     __syncthreads();
     int mt_idx = 624;
 
     if (warp == 0)
-        for (unsigned long long i = 0; i < a.N1; ++i) draw_read(a, i, false, counts, z, s_arr, g_arr, mt, mt_idx, lane);
+        for (unsigned long long i = 0; i < a.N1; ++i) draw_read(a, i, false, counts, z, s_arr, g_arr, mt, mt_idx, lane, err);
     __syncthreads();
 
     const int chainlen = 1 + (n_samples - 1) * a.gap;
     int kept = 0;
     for (int round = 1; round <= a.burnin + chainlen; ++round) {
         if (warp == 0)
-            for (unsigned long long i = 0; i < a.N1; ++i) draw_read(a, i, true, counts, z, s_arr, g_arr, mt, mt_idx, lane);
+            for (unsigned long long i = 0; i < a.N1; ++i) draw_read(a, i, true, counts, z, s_arr, g_arr, mt, mt_idx, lane, err);
         __syncthreads();
-        if (round > a.burnin && (round - a.burnin - 1) % a.gap == 0) {  // Gibbs.cpp:313-346
-            // count vector + theta = (c + alpha) / totc, zero for omitted; polishTheta; TPM / FPKM
-            double part = 0.0;
-            for (int i = tid; i < M1; i += blockDim.x) {
-                const int c = counts[i];
-                cv[(size_t)kept * M1 + i] = c;
-                double th = c < 0 ? 0.0 : ((double)c + a.alpha[i]) / a.totc;
-                if (i > 0 && (a.mw[i] < kEpsilon || a.eel[i] < kEpsilon)) th = 0.0;
-                else th = th / a.mw[i];
-                theta[i] = th;
-                part += th;
-            }
-            const double tsum = block_sum(part, sh_red);
-            part = 0.0;
-            for (int i = tid; i < M1; i += blockDim.x) {
-                const double th = theta[i] / tsum;
-                theta[i] = th;
-                if (i > 0 && a.eel[i] >= kEpsilon) part += th;
-            }
-            double denom = block_sum(part, sh_red);
-            if (denom < kEpsilon) denom = 1.0;
-            part = 0.0;
-            for (int i = tid; i < M1; i += blockDim.x) {
-                const double f = (i > 0 && a.eel[i] >= kEpsilon) ? (theta[i] / denom) * 1e9 / a.eel[i] : 0.0;
-                fpkm[i] = f;
-                part += f;
-            }
-            double fsum = block_sum(part, sh_red);
-            if (fsum < kEpsilon) fsum = 1.0;
-            for (int i = tid; i < M1; i += blockDim.x) {
-                const double c = (double)counts[i];
-                acc[i] += c;
-                acc[M1 + i] += c * c;
-                acc[2 * (size_t)M1 + i] += i > 0 ? fpkm[i] / fsum * 1e6 : 0.0;
-                acc[3 * (size_t)M1 + i] += fpkm[i];
-            }
-            for (int gi = tid; gi < a.n_genes; gi += blockDim.x) {
-                double c = 0.0;
-                for (int j = a.gene_start[gi]; j < a.gene_start[gi + 1]; ++j) c += counts[j];
-                acc[4 * (size_t)M1 + gi] += c * c;
-            }
+        if (round > a.burnin && (round - a.burnin - 1) % a.gap == 0) {
+            keep_sample(a, counts, cv, acc, theta, kept, tid, M1, sh_red);
             ++kept;
             __syncthreads();
         }
@@ -248,7 +285,7 @@ __global__ void __launch_bounds__(kGibbsThreads) gibbs_chain_kernel(const GibbsA
 // read x transcript graph (noise transcript 0 excluded) touch disjoint counts and commute exactly.  The only
 // global coupling is the noise count c0 = counts[0], which enters every row that has a noise entry.
 //
-//   * Static, once per upload (gibbs_prepare, host): connected components (union-find over transcripts); the reads
+//   * Static, once per upload (gibbs_layout, host): connected components (union-find over transcripts); the reads
 //     grouped by component in read order ("segments", longest first); rows re-laid in that slot order.
 //   * A sweep of a chain: every segment is walked by ONE group of 16 lanes in read order with the live counts of its
 //     component (component-private: registers for components of < 32 transcripts, L2 otherwise).  The noise count read i must see is c0(i) = c0 at the start of the
@@ -267,20 +304,7 @@ __global__ void __launch_bounds__(kGibbsThreads) gibbs_chain_kernel(const GibbsA
 //     workers meet at a per-chain barrier in global memory a handful of times per sweep (not once per block of reads);
 //     chains never synchronise with each other.
 // ================================================================================================
-constexpr int kPThreads = 256;
-
-struct ChainSync {
-    unsigned count, gen;        // barrier among the chain's worker CTAs
-    unsigned u_ready;           // generator -> workers: uniforms of sweeps < u_ready are complete
-    unsigned sweeps_done;       // workers -> generator: sweeps < sweeps_done no longer need their uniform buffer
-    unsigned changed;           // some flip word differs between the pass's input and output sets
-    unsigned next_seg;          // next component to be claimed in the current pass
-    int err;
-    unsigned passes;            // diagnostics: passes run over all sweeps
-    unsigned long long prof[4]; // clock64 totals of worker CTA 0: wait for uniforms, passes, barriers + bookkeeping, per-sample work
-};
-
-struct PArgs {
+struct PArgs : RunArgs {
     unsigned long long N1;
     const int* order;                   // read id of slot q (component by component, read order inside)
     const unsigned long long* p_off;    // N1 + 1 entry offsets of the slots, rows stored in slot order
@@ -292,16 +316,7 @@ struct PArgs {
     const int* comp_tids;
     int n_segs;
     int fast_rows;                      // converged walk: lean code path for rows of register-resident components
-    int M, burnin, gap, n_genes, n_chains, ctas_per_chain, chain_base;
-    const int* chain_samples;
-    const unsigned* chain_seeds;
-    const long long* chain_cv_offset;
-    double n0, totc;
-    const int* init_counts;
-    const double* alpha;
-    const double* eel;
-    const double* mw;
-    const int* gene_start;
+    int n_chains, ctas_per_chain, chain_base;
     int* counts;           // n_chains * (M + 1)
     int* counts_start;     // n_chains * (M + 1): copy taken at the start of a sweep
     int* z;                // n_chains * 2 * N1, indexed by SLOT; [sweep parity]
@@ -310,14 +325,7 @@ struct PArgs {
     int* pre;              // n_chains * W: net flips in the words before w inside its CTA slice
     int* slice_tot;        // n_chains * ctas_per_chain: net flips of every CTA slice
     unsigned n_words;      // W = ceil(N1 / 32)
-    ChainSync* sync;       // n_chains
-    int* count_vectors;
-    double* acc;
-    double* theta_tmp;
 };
-
-__device__ __forceinline__ int ld_cg(const int* p) { return __ldcg(p); }
-__device__ __forceinline__ void st_cg(int* p, int v) { __stcg(p, v); }
 
 __device__ void chain_barrier(ChainSync* s, unsigned n_ctas) {
     __syncthreads();
@@ -343,10 +351,7 @@ __device__ void chain_barrier(ChainSync* s, unsigned n_ctas) {
 __device__ void generator_loop(const PArgs& a, ChainSync* sy, unsigned* ubuf, unsigned n_sweeps, unsigned seed) {
     __shared__ unsigned st[2][624];
     const unsigned tid = threadIdx.x;
-    if (tid == 0) {  // init_genrand (boost mt19937 seeding)
-        st[0][0] = seed;
-        for (int k = 1; k < 624; ++k) st[0][k] = 1812433253u * (st[0][k - 1] ^ (st[0][k - 1] >> 30)) + (unsigned)k;
-    }
+    if (tid == 0) mt_seed(st[0], seed);
     __syncthreads();
     int cur = 0;
     const unsigned long long total = (unsigned long long)n_sweeps * a.N1;
@@ -943,7 +948,6 @@ __device__ __forceinline__ void chain_body(const PArgs& a, const int chain, cons
     int* slice_tot = a.slice_tot + (size_t)chain * n_ctas;
     double* acc = a.acc + (size_t)chain * (4 * (size_t)M1 + a.n_genes);
     double* theta = a.theta_tmp + slot * 2 * M1;
-    double* fpkm = theta + M1;
     int* cv = a.count_vectors + a.chain_cv_offset[chain] * M1;
     // this CTA's slice of flip words (prefix sums are formed per slice, the slice bases are added on the fly)
     const unsigned w_per = (W + n_ctas - 1) / n_ctas;
@@ -1080,48 +1084,8 @@ __device__ __forceinline__ void chain_body(const PArgs& a, const int chain, cons
             __threadfence();
             atomicExch(&sy->sweeps_done, sweep + 1);   // this sweep's uniforms (and the previous z) are no longer read
         }
-        if (round > a.burnin && (round - a.burnin - 1) % a.gap == 0) {   // Gibbs.cpp:313-346, by CTA 0 of the chain
-            if (cta == 0) {
-                double part = 0.0;
-                for (int i = tid; i < M1; i += kPThreads) {
-                    const int c = ld_cg(counts + i);
-                    cv[(size_t)kept * M1 + i] = c;
-                    double th = c < 0 ? 0.0 : ((double)c + a.alpha[i]) / a.totc;
-                    if (i > 0 && (a.mw[i] < kEpsilon || a.eel[i] < kEpsilon)) th = 0.0;
-                    else th = th / a.mw[i];
-                    theta[i] = th;
-                    part += th;
-                }
-                const double tsum = block_sum(part, sh_red);
-                part = 0.0;
-                for (int i = tid; i < M1; i += kPThreads) {
-                    const double th = theta[i] / tsum;
-                    theta[i] = th;
-                    if (i > 0 && a.eel[i] >= kEpsilon) part += th;
-                }
-                double denom = block_sum(part, sh_red);
-                if (denom < kEpsilon) denom = 1.0;
-                part = 0.0;
-                for (int i = tid; i < M1; i += kPThreads) {
-                    const double f = (i > 0 && a.eel[i] >= kEpsilon) ? (theta[i] / denom) * 1e9 / a.eel[i] : 0.0;
-                    fpkm[i] = f;
-                    part += f;
-                }
-                double fsum = block_sum(part, sh_red);
-                if (fsum < kEpsilon) fsum = 1.0;
-                for (int i = tid; i < M1; i += kPThreads) {
-                    const double c = (double)ld_cg(counts + i);
-                    acc[i] += c;
-                    acc[M1 + i] += c * c;
-                    acc[2 * (size_t)M1 + i] += i > 0 ? fpkm[i] / fsum * 1e6 : 0.0;
-                    acc[3 * (size_t)M1 + i] += fpkm[i];
-                }
-                for (int gi = tid; gi < a.n_genes; gi += kPThreads) {
-                    double c = 0.0;
-                    for (int j = a.gene_start[gi]; j < a.gene_start[gi + 1]; ++j) c += ld_cg(counts + j);
-                    acc[4 * (size_t)M1 + gi] += c * c;
-                }
-            }
+        if (round > a.burnin && (round - a.burnin - 1) % a.gap == 0) {   // by CTA 0 of the chain
+            if (cta == 0) keep_sample(a, counts, cv, acc, theta, kept, tid, M1, sh_red);
             ++kept;
             chain_barrier(sy, n_ctas);
         }
@@ -1201,11 +1165,218 @@ __global__ void __launch_bounds__(kPThreads, 3) gibbs_batch_kernel(const BArgs b
     }
 }
 
-template <class T>
-int to_dev(T** d, const T* h, size_t n, cudaStream_t s) {
-    RB_CUDA(cudaMalloc(d, std::max<size_t>(n, 1) * sizeof(T)));
-    if (n) RB_CUDA(cudaMemcpyAsync(*d, h, n * sizeof(T), cudaMemcpyHostToDevice, s));
+// ---- host side: the device blocks of a sample ----------------------------------------------------------------------------
+constexpr int kBatchMaxWorkers = 8;   // worker CTAs per K13 team; a batch sample's slice totals are sized for it
+constexpr int kBatchDefaultWorkers = 2;
+
+size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// lays parts out one behind the other, each on a 256-byte boundary
+struct Packer {
+    size_t at = 0;
+    size_t put(size_t bytes) {
+        const size_t off = at;
+        at = align_up(at + bytes);
+        return off;
+    }
+};
+
+// Byte offsets of the two parts of a sample, each from its own start.
+//   layout part: the component layout (n_segs <= N1 and comp_tids <= M + 1 bound it before it is built), then the CSR
+//     rows the serial kernel reads (`csr`: a context's upload; a batch sample has none);
+//   run part: the inputs of a run up to `zero`; the chain states, the slice totals (`workers` per chain) and the sums,
+//     zeroed before the run, up to `cv`; then the count vectors.
+// A batch sample keeps both in one block, the run part behind the layout part; a context keeps the layout part from its
+// upload and the run part of each rsem_b200_gibbs_run_chains call in blocks of their own.
+struct GParts {
+    size_t order, p_off, p_sid, p_con, seg_start, seg_ntr, seg_tid_off, comp_tids, row_ptr, sid, conprb, layout;
+    size_t init, alpha, eel, mw, gene, samples, seeds, cv_off, zero, sync, slice_tot, acc, cv, run;
+};
+GParts gparts(uint64_t N1, uint64_t E, int M, bool csr, int n_genes, int64_t n_samples, int n_chains, int workers) {
+    const size_t M1 = (size_t)M + 1, nc = (size_t)n_chains;
+    GParts p{};
+    Packer k;
+    p.order = k.put(N1 * 4);
+    p.p_off = k.put((N1 + 1) * 8);
+    p.p_sid = k.put((E + 16) * 4);
+    p.p_con = k.put((E + 16) * 8);
+    p.seg_start = k.put((N1 + 1) * 4);
+    p.seg_ntr = k.put(std::max<uint64_t>(N1, 1) * 4);
+    p.seg_tid_off = k.put((N1 + 1) * 4);
+    p.comp_tids = k.put((M1 + 1) * 4);
+    p.row_ptr = k.put(csr ? (N1 + 1) * 8 : 0);
+    p.sid = k.put(csr ? (E + 4) * 4 : 0);
+    p.conprb = k.put(csr ? (E + 4) * 8 : 0);
+    p.layout = k.at;
+    k.at = 0;
+    p.init = k.put(M1 * 4);
+    p.alpha = k.put(M1 * 8);
+    p.eel = k.put(M1 * 8);
+    p.mw = k.put(M1 * 8);
+    p.gene = k.put(((size_t)n_genes + 1) * 4);
+    p.samples = k.put(nc * 4);
+    p.seeds = k.put(nc * 4);
+    p.cv_off = k.put(nc * 8);
+    p.zero = k.at;
+    p.sync = k.put(nc * sizeof(ChainSync));
+    p.slice_tot = k.put(nc * workers * 4);
+    p.acc = k.put(nc * (4 * M1 + (size_t)n_genes) * 8);
+    p.cv = k.put((size_t)n_samples * M1 * 4);
+    p.run = k.at;
+    return p;
+}
+
+// Byte offsets of the scratch `teams` chains run in (a chain of rsem_b200_gibbs_run_chains, a team of K13), for up to n1
+// reads: counts, their copy at the start of a sweep, z and the uniforms [sweep parity], flip words [set][joined / left],
+// their prefix, theta / fpkm, and the serial kernel's cumulative arrays of rows longer than kRowCap (row_len doubles).
+struct Scratch {
+    size_t counts, counts_start, z, ubuf, flips, pre, theta, row, total;
+};
+Scratch scratch_parts(size_t M1, uint64_t n1, size_t teams, uint64_t row_len) {
+    const size_t W = (n1 + 31) / 32;
+    Scratch s{};
+    Packer k;
+    s.counts = k.put(teams * M1 * 4);
+    s.counts_start = k.put(teams * M1 * 4);
+    s.z = k.put(teams * 2 * n1 * 4);
+    s.ubuf = k.put(teams * 2 * n1 * 4);
+    s.flips = k.put(teams * 4 * W * 4);
+    s.pre = k.put(teams * W * 4);
+    s.theta = k.put(teams * 2 * M1 * 8);
+    s.row = k.put(teams * row_len * 8);
+    s.total = k.at;
+    return s;
+}
+
+void put(unsigned char* img, size_t off, const void* src, size_t n) {
+    if (n) memcpy(img + off, src, n);
+}
+
+// Writes the component layout, p_con excepted, through put(offset in the layout part, source, bytes): into a host image
+// (K13) or straight to the device (a context's upload).
+template <class Put>
+void pack_layout(Put put, const GParts& q, const GibbsLayout& L) {
+    put(q.order, L.order.data(), L.order.size() * 4);
+    put(q.p_off, L.p_off.data(), L.p_off.size() * 8);
+    put(q.p_sid, L.p_sid.data(), L.p_sid.size() * 4);
+    put(q.seg_start, L.seg_start.data(), L.seg_start.size() * 4);
+    put(q.seg_ntr, L.seg_ntr.data(), L.seg_ntr.size() * 4);
+    put(q.seg_tid_off, L.seg_tid_off.data(), L.seg_tid_off.size() * 4);
+    put(q.comp_tids, L.comp_tids.data(), L.comp_tids.size() * 4);
+}
+
+// host image of the inputs of a run: [0, q.zero) of the run part
+void pack_run(unsigned char* img, const GParts& q, const rsem_b200_gibbs_params* p) {
+    const size_t M1 = (size_t)p->M + 1, nc = (size_t)p->n_chains;
+    put(img, q.init, p->init_counts, M1 * 4);
+    put(img, q.alpha, p->pseudo_counts, M1 * 8);
+    put(img, q.eel, p->eel, M1 * 8);
+    put(img, q.mw, p->mw, M1 * 8);
+    put(img, q.gene, p->gene_start, ((size_t)p->n_genes + 1) * 4);
+    put(img, q.samples, p->chain_samples, nc * 4);
+    put(img, q.seeds, p->chain_seeds, nc * 4);
+    long long* off = reinterpret_cast<long long*>(img + q.cv_off);
+    long long at = 0;
+    for (size_t t = 0; t < nc; ++t) { off[t] = at; at += p->chain_samples[t]; }
+}
+
+int64_t total_samples(const rsem_b200_gibbs_params* p) {
+    int64_t n = 0;
+    for (int t = 0; t < p->n_chains; ++t) n += p->chain_samples[t];
+    return n;
+}
+
+// typed pointers into a layout part at `base`
+GibbsView layout_view(void* base, const GParts& q) {
+    const unsigned char* b = static_cast<const unsigned char*>(base);
+    GibbsView v;
+    v.order = reinterpret_cast<const int32_t*>(b + q.order);
+    v.p_off = reinterpret_cast<const uint64_t*>(b + q.p_off);
+    v.p_sid = reinterpret_cast<const int32_t*>(b + q.p_sid);
+    v.p_con = reinterpret_cast<const double*>(b + q.p_con);
+    v.seg_start = reinterpret_cast<const int32_t*>(b + q.seg_start);
+    v.seg_ntr = reinterpret_cast<const int32_t*>(b + q.seg_ntr);
+    v.seg_tid_off = reinterpret_cast<const int32_t*>(b + q.seg_tid_off);
+    v.comp_tids = reinterpret_cast<const int32_t*>(b + q.comp_tids);
+    v.row_ptr = reinterpret_cast<const uint64_t*>(b + q.row_ptr);
+    v.sid = reinterpret_cast<const int32_t*>(b + q.sid);
+    v.conprb = reinterpret_cast<const double*>(b + q.conprb);
+    return v;
+}
+
+// the component layout fields of the walks' arguments
+void set_layout(PArgs& a, const GibbsView& v, uint64_t N1, int n_segs) {
+    a.N1 = N1;
+    a.order = v.order;
+    a.p_off = reinterpret_cast<const unsigned long long*>(v.p_off);
+    a.p_sid = v.p_sid;
+    a.p_con = v.p_con;
+    a.seg_start = v.seg_start;
+    a.seg_ntr = v.seg_ntr;
+    a.seg_tid_off = v.seg_tid_off;
+    a.comp_tids = v.comp_tids;
+    a.n_segs = n_segs;
+    a.n_words = (unsigned)((N1 + 31) / 32);
+}
+
+// what the kernels read about a run whose run part is at `run` (device memory); theta_tmp is the caller's scratch
+RunArgs run_args(unsigned char* run, const GParts& q, const rsem_b200_gibbs_params* p, double* theta_tmp) {
+    RunArgs a;
+    a.M = p->M; a.burnin = p->burnin; a.gap = p->gap; a.n_genes = p->n_genes;
+    a.chain_samples = reinterpret_cast<const int*>(run + q.samples);
+    a.chain_seeds = reinterpret_cast<const unsigned*>(run + q.seeds);
+    a.chain_cv_offset = reinterpret_cast<const long long*>(run + q.cv_off);
+    a.n0 = p->n0; a.totc = p->totc;
+    a.init_counts = reinterpret_cast<const int*>(run + q.init);
+    a.alpha = reinterpret_cast<const double*>(run + q.alpha);
+    a.eel = reinterpret_cast<const double*>(run + q.eel);
+    a.mw = reinterpret_cast<const double*>(run + q.mw);
+    a.gene_start = reinterpret_cast<const int*>(run + q.gene);
+    a.count_vectors = reinterpret_cast<int*>(run + q.cv);
+    a.acc = reinterpret_cast<double*>(run + q.acc);
+    a.theta_tmp = theta_tmp;
+    a.sync = reinterpret_cast<ChainSync*>(run + q.sync);
+    return a;
+}
+
+// the block of one rsem_b200_gibbs_run_chains call: its run part with `scratch` bytes behind it
+struct RunBlock {
+    unsigned char* p = nullptr;
+    ~RunBlock() { cudaFree(p); }
+};
+int upload_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, const GParts& q, size_t scratch, RunBlock& b) {
+    std::vector<unsigned char> img(q.zero, 0);
+    pack_run(img.data(), q, p);
+    RB_CUDA(cudaMalloc(&b.p, q.run + scratch));
+    RB_CUDA(cudaMemcpyAsync(b.p, img.data(), q.zero, cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMemsetAsync(b.p + q.zero, 0, q.cv - q.zero, c->stream));   // chain states, slice totals, sums
+    RB_CUDA(cudaStreamSynchronize(c->stream));   // img goes out of scope
     return 0;
+}
+
+// Copies the sums, the count vectors and the chain states of the run part at `run` to the host, each one whose destination
+// is given.  A chain whose categorical draw fell off its cumulative array fails the run.
+int read_run(rsem_b200_ctx* c, const unsigned char* run, const GParts& q, int n_chains, int64_t n_samples, int M, int n_genes,
+             int32_t* count_vectors, double* chain_acc, ChainSync* sync) {
+    const size_t M1 = (size_t)M + 1;
+    if (chain_acc)
+        RB_CUDA(cudaMemcpyAsync(chain_acc, run + q.acc, (size_t)n_chains * (4 * M1 + n_genes) * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (count_vectors)
+        RB_CUDA(cudaMemcpyAsync(count_vectors, run + q.cv, (size_t)n_samples * M1 * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (sync) RB_CUDA(cudaMemcpyAsync(sync, run + q.sync, (size_t)n_chains * sizeof(ChainSync), cudaMemcpyDeviceToHost, c->stream));
+    RB_CUDA(cudaStreamSynchronize(c->stream));
+    for (int t = 0; sync && t < n_chains; ++t)
+        if (sync[t].err) {
+            set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
+            return RSEM_B200_ERR_ARG;
+        }
+    return 0;
+}
+
+// a row without entries has nothing to draw from (every kernel would fall off its empty cumulative array)
+int refuse_empty_row() {
+    set_error("gibbs: a read without any entry (the .ofg writer never emits one)");
+    return RSEM_B200_ERR_ARG;
 }
 
 }  // namespace
@@ -1213,97 +1384,41 @@ int to_dev(T** d, const T* h, size_t n, cudaStream_t s) {
 static int gibbs_run_serial(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
                             rsem_b200_gibbs_stats* stats) {
     const DevGibbs& g = c->gibbs;
-    const int M1 = p->M + 1, nc = p->n_chains;
-    long long total_samples = 0;
-    std::vector<long long> cv_off(nc);
-    for (int t = 0; t < nc; ++t) { cv_off[t] = total_samples; total_samples += p->chain_samples[t]; }
-
-    // longest row decides whether the cumulative array fits shared memory
-    std::vector<uint64_t> h_rp(g.N1 + 1);
-    RB_CUDA(cudaMemcpyAsync(h_rp.data(), g.row_ptr, (g.N1 + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
-    uint64_t max_len = 1;
-    for (uint64_t i = 0; i < g.N1; ++i) max_len = std::max(max_len, h_rp[i + 1] - h_rp[i]);
+    const int nc = p->n_chains;
+    const int64_t n_samples = total_samples(p);
+    const GParts q = gparts(g.N1, g.E, p->M, false, p->n_genes, n_samples, nc, 0);
+    const uint64_t row_len = g.max_len > kRowCap ? g.max_len : 0;   // the longest row decides whether shared memory holds it
+    const Scratch s = scratch_parts((size_t)p->M + 1, g.N1, nc, row_len);
+    RunBlock run;
+    if (int rc = upload_run(c, p, q, s.total, run)) return rc;
+    unsigned char* sb = run.p + q.run;
 
     GibbsArgs a{};
+    static_cast<RunArgs&>(a) = run_args(run.p, q, p, reinterpret_cast<double*>(sb + s.theta));
     a.N1 = g.N1;
-    a.row_ptr = reinterpret_cast<const unsigned long long*>(g.row_ptr);
-    a.sid = g.sid;
-    a.conprb = g.conprb;
-    a.M = p->M; a.burnin = p->burnin; a.gap = p->gap; a.n_genes = p->n_genes;
-    a.n0 = p->n0; a.totc = p->totc;
-    a.max_len = (unsigned)max_len;
-    a.err_flag = c->err_flag;
-
-    int *d_samples = nullptr, *d_init = nullptr, *d_gene = nullptr, *d_counts = nullptr, *d_z = nullptr, *d_cv = nullptr;
-    unsigned* d_seeds = nullptr;
-    long long* d_off = nullptr;
-    double *d_alpha = nullptr, *d_eel = nullptr, *d_mw = nullptr, *d_scratch = nullptr, *d_acc = nullptr, *d_tmp = nullptr;
-    const size_t acc_per = 4 * (size_t)M1 + p->n_genes;
-    int rc = 0;
-    auto cleanup = [&]() {
-        cudaFree(d_samples); cudaFree(d_init); cudaFree(d_gene); cudaFree(d_counts); cudaFree(d_z); cudaFree(d_cv);
-        cudaFree(d_seeds); cudaFree(d_off); cudaFree(d_alpha); cudaFree(d_eel); cudaFree(d_mw); cudaFree(d_scratch);
-        cudaFree(d_acc); cudaFree(d_tmp);
-    };
-#define RB_TRY(x) do { rc = (x); if (rc) { cleanup(); return rc; } } while (0)
-#define RB_TRYC(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { cleanup(); return cuda_fail(e_, #x, __FILE__, __LINE__); } } while (0)
-    RB_TRY(to_dev(&d_samples, p->chain_samples, nc, c->stream));
-    RB_TRY(to_dev(&d_seeds, p->chain_seeds, nc, c->stream));
-    RB_TRY(to_dev(&d_off, cv_off.data(), nc, c->stream));
-    RB_TRY(to_dev(&d_init, p->init_counts, M1, c->stream));
-    RB_TRY(to_dev(&d_alpha, p->pseudo_counts, M1, c->stream));
-    RB_TRY(to_dev(&d_eel, p->eel, M1, c->stream));
-    RB_TRY(to_dev(&d_mw, p->mw, M1, c->stream));
-    RB_TRY(to_dev(&d_gene, p->gene_start, (size_t)p->n_genes + 1, c->stream));
-    RB_TRYC(cudaMalloc(&d_counts, (size_t)nc * M1 * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_z, std::max<size_t>((size_t)nc * g.N1, 1) * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_cv, std::max<size_t>((size_t)total_samples * M1, 1) * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_acc, (size_t)nc * acc_per * sizeof(double)));
-    RB_TRYC(cudaMalloc(&d_tmp, (size_t)nc * 2 * M1 * sizeof(double)));
-    RB_TRYC(cudaMemsetAsync(d_acc, 0, (size_t)nc * acc_per * sizeof(double), c->stream));
-    if (max_len > kRowCap) RB_TRYC(cudaMalloc(&d_scratch, (size_t)nc * max_len * sizeof(double)));
-    a.chain_samples = d_samples; a.chain_seeds = d_seeds; a.chain_cv_offset = d_off; a.init_counts = d_init;
-    a.alpha = d_alpha; a.eel = d_eel; a.mw = d_mw; a.gene_start = d_gene; a.counts = d_counts; a.z = d_z;
-    a.scratch = d_scratch; a.count_vectors = d_cv; a.acc = d_acc; a.theta_tmp = d_tmp;
+    a.row_ptr = reinterpret_cast<const unsigned long long*>(g.v.row_ptr);
+    a.sid = g.v.sid;
+    a.conprb = g.v.conprb;
+    a.counts = reinterpret_cast<int*>(sb + s.counts);
+    a.z = reinterpret_cast<int*>(sb + s.z);
+    a.scratch = reinterpret_cast<double*>(sb + s.row);
+    a.max_len = (unsigned)row_len;
 
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     if (stats) { cudaEventCreate(&ev0); cudaEventCreate(&ev1); cudaEventRecord(ev0, c->stream); }
     gibbs_chain_kernel<<<nc, kGibbsThreads, 0, c->stream>>>(a);
-    RB_TRYC(cudaGetLastError());
+    RB_CUDA(cudaGetLastError());
     c->launches++;
     if (stats) cudaEventRecord(ev1, c->stream);
-
-    RB_TRYC(cudaMemcpyAsync(chain_acc, d_acc, (size_t)nc * acc_per * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaMemcpyAsync(count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    int err = 0;
-    RB_TRYC(cudaMemcpyAsync(&err, c->err_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaStreamSynchronize(c->stream));
-    cleanup();
-#undef RB_TRY
-#undef RB_TRYC
+    std::vector<ChainSync> sync(nc);
+    const int rc = read_run(c, run.p, q, nc, n_samples, p->M, p->n_genes, count_vectors, chain_acc, sync.data());
     if (stats) {
         float ms = 0;
         cudaEventElapsedTime(&ms, ev0, ev1);
         cudaEventDestroy(ev0); cudaEventDestroy(ev1);
         *stats = rsem_b200_gibbs_stats{ms, 0, 1};
     }
-    if (err) {
-        cudaMemset(c->err_flag, 0, sizeof(int));
-        set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
-        return RSEM_B200_ERR_ARG;
-    }
-    return 0;
-}
-
-
-__global__ void permute_rows_kernel(const unsigned long long* row_ptr, const double* conprb, const int* order,
-                                    const unsigned long long* p_off, unsigned long long N1, double* p_con) {
-    for (unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; q < N1;
-         q += (unsigned long long)gridDim.x * blockDim.x) {
-        const unsigned long long src = row_ptr[order[q]], dst = p_off[q], n = p_off[q + 1] - dst;
-        for (unsigned long long k = 0; k < n; ++k) p_con[dst + k] = conprb[src + k];
-    }
+    return rc;
 }
 
 // ---- static preparation for the component-parallel sampler (host) ---------------------------------------------
@@ -1403,62 +1518,59 @@ int gibbs_layout(const uint64_t* row_ptr, const int32_t* sid, uint64_t N1, int M
     return 0;
 }
 
-int gibbs_prepare(rsem_b200_ctx* c, const uint64_t* row_ptr, const int32_t* sid) {
-    DevGibbs& g = c->gibbs;
-    const uint64_t N1 = g.N1;
-    if (N1 == 0) return 0;
+GibbsView gibbs_view(void* block, uint64_t N1, uint64_t E, int M) {
+    return layout_view(block, gparts(N1, E, M, true, 0, 0, 0, 0));
+}
+
+__global__ void permute_rows_kernel(const unsigned long long* row_ptr, const double* conprb, const int* order,
+                                    const unsigned long long* p_off, unsigned long long N1, double* p_con) {
+    for (unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; q < N1;
+         q += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long src = row_ptr[order[q]], dst = p_off[q], n = p_off[q + 1] - dst;
+        for (unsigned long long k = 0; k < n; ++k) p_con[dst + k] = conprb[src + k];
+    }
+}
+
+int gibbs_upload(rsem_b200_ctx* c, uint64_t N1, uint64_t E, int M, const uint64_t* row_ptr, const int32_t* sid, const double* conprb) {
     GibbsLayout L;
-    if (int rc = gibbs_layout(row_ptr, sid, N1, g.M, L)) return rc;
+    if (int rc = gibbs_layout(row_ptr, sid, N1, M, L)) return rc;
+    const GParts q = gparts(N1, E, M, true, 0, 0, 0, 0);
+    DevGibbs& g = c->gibbs;
+    RB_CUDA(cudaMalloc(&g.block, q.layout));
+    g.bytes = q.layout;
+    unsigned char* base = static_cast<unsigned char*>(g.block);
+    cudaError_t e = cudaSuccess;
+    auto put = [&](size_t off, const void* src, size_t n) {
+        if (n && e == cudaSuccess) e = cudaMemcpyAsync(base + off, src, n, cudaMemcpyHostToDevice, c->stream);
+    };
+    pack_layout(put, q, L);
+    put(q.row_ptr, row_ptr, (N1 + 1) * 8);
+    put(q.sid, sid, E * 4);
+    put(q.conprb, conprb, E * 8);
+    RB_CUDA(e);
+    g.v = layout_view(g.block, q);
+    // conprb in slot order, permuted on the device from the uploaded copy
+    permute_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(reinterpret_cast<const unsigned long long*>(g.v.row_ptr), g.v.conprb,
+                                                               g.v.order, reinterpret_cast<const unsigned long long*>(g.v.p_off), N1,
+                                                               const_cast<double*>(g.v.p_con));
+    RB_CUDA(cudaGetLastError());
+    c->launches++;
+    RB_CUDA(cudaStreamSynchronize(c->stream));   // L goes out of scope
+    g.N1 = N1;
+    g.E = E;
+    g.M = M;
+    g.n_segs = L.n_segs;
     g.max_len = L.max_len;
     g.empty_row = L.empty_row;
-    g.n_segs = L.n_segs;
-    {
-        const uint64_t E = row_ptr[N1];
-        RB_CUDA(cudaMalloc(&g.p_off, (N1 + 1) * sizeof(uint64_t)));
-        RB_CUDA(cudaMalloc(&g.p_sid, (E + 16) * sizeof(int32_t)));
-        RB_CUDA(cudaMalloc(&g.p_con, (E + 16) * sizeof(double)));
-        RB_CUDA(cudaMemcpyAsync(g.p_off, L.p_off.data(), (N1 + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
-        RB_CUDA(cudaMemcpyAsync(g.p_sid, L.p_sid.data(), E * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-        // conprb is permuted on the device from the already uploaded copy
-        RB_CUDA(cudaMalloc(&g.order, N1 * sizeof(int32_t)));
-        RB_CUDA(cudaMemcpyAsync(g.order, L.order.data(), N1 * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-        permute_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(reinterpret_cast<const unsigned long long*>(g.row_ptr), g.conprb,
-                                                                   g.order, reinterpret_cast<const unsigned long long*>(g.p_off), N1, g.p_con);
-        RB_CUDA(cudaGetLastError());
-        c->launches++;
-        RB_CUDA(cudaStreamSynchronize(c->stream));
-    }
-    RB_CUDA(cudaMalloc(&g.seg_start, L.seg_start.size() * sizeof(int32_t)));
-    RB_CUDA(cudaMemcpyAsync(g.seg_start, L.seg_start.data(), L.seg_start.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMalloc(&g.seg_ntr, std::max<size_t>(L.seg_ntr.size(), 1) * sizeof(int32_t)));
-    RB_CUDA(cudaMalloc(&g.seg_tid_off, L.seg_tid_off.size() * sizeof(int32_t)));
-    RB_CUDA(cudaMalloc(&g.comp_tids, L.comp_tids.size() * sizeof(int32_t)));
-    g.n_comp_tids = L.comp_tids.size();
-    RB_CUDA(cudaMemcpyAsync(g.seg_ntr, L.seg_ntr.data(), L.seg_ntr.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(g.seg_tid_off, L.seg_tid_off.data(), L.seg_tid_off.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemcpyAsync(g.comp_tids, L.comp_tids.data(), L.comp_tids.size() * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
+    g.ready = true;
     return 0;
 }
 
 static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
                               rsem_b200_gibbs_stats* stats) {
     const DevGibbs& g = c->gibbs;
-    const int M1 = p->M + 1, nc = p->n_chains;
-    long long total_samples = 0;
-    std::vector<long long> cv_off(nc);
-    for (int t = 0; t < nc; ++t) { cv_off[t] = total_samples; total_samples += p->chain_samples[t]; }
-    const size_t acc_per = 4 * (size_t)M1 + p->n_genes;
-    const unsigned W = (unsigned)((g.N1 + 31) / 32);
-
-    PArgs a{};
-    a.N1 = g.N1;
-    a.order = g.order; a.seg_start = g.seg_start; a.n_segs = g.n_segs;
-    a.seg_ntr = g.seg_ntr; a.seg_tid_off = g.seg_tid_off; a.comp_tids = g.comp_tids;
-    a.p_off = reinterpret_cast<const unsigned long long*>(g.p_off); a.p_sid = g.p_sid; a.p_con = g.p_con;
-    a.M = p->M; a.burnin = p->burnin; a.gap = p->gap; a.n_genes = p->n_genes; a.n_chains = nc;
-    a.n0 = p->n0; a.totc = p->totc;
-    a.n_words = W;
+    const int nc = p->n_chains;
+    const int64_t n_samples = total_samples(p);
 
     // co-resident CTAs: chains run in waves, every chain gets the same number of worker CTAs (one lane group per component
     // is all the parallelism a sweep has) + 1 generator CTA
@@ -1475,47 +1587,23 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
     ctas = std::min(ctas, std::max(1, resident / std::min(nc, std::max(1, resident / 2)) - 1));
     const int chains_per_wave = std::max(1, std::min(nc, resident / (ctas + 1)));
 
-    int *d_samples = nullptr, *d_init = nullptr, *d_gene = nullptr, *d_counts = nullptr, *d_counts0 = nullptr, *d_z = nullptr, *d_cv = nullptr,
-        *d_pre = nullptr, *d_tot = nullptr;
-    unsigned *d_seeds = nullptr, *d_u = nullptr, *d_flips = nullptr;
-    long long* d_off = nullptr;
-    ChainSync* d_sync = nullptr;
-    double *d_alpha = nullptr, *d_eel = nullptr, *d_mw = nullptr, *d_acc = nullptr, *d_tmp = nullptr;
-    int rc = 0;
-    auto cleanup = [&]() {
-        cudaFree(d_samples); cudaFree(d_init); cudaFree(d_gene); cudaFree(d_counts); cudaFree(d_counts0); cudaFree(d_z); cudaFree(d_cv);
-        cudaFree(d_pre); cudaFree(d_tot); cudaFree(d_seeds); cudaFree(d_u); cudaFree(d_flips); cudaFree(d_off); cudaFree(d_sync);
-        cudaFree(d_alpha); cudaFree(d_eel); cudaFree(d_mw); cudaFree(d_acc); cudaFree(d_tmp);
-    };
-#define RB_TRY(x) do { rc = (x); if (rc) { cleanup(); return rc; } } while (0)
-#define RB_TRYC(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { cleanup(); return cuda_fail(e_, #x, __FILE__, __LINE__); } } while (0)
-    RB_TRY(to_dev(&d_samples, p->chain_samples, nc, c->stream));
-    RB_TRY(to_dev(&d_seeds, p->chain_seeds, nc, c->stream));
-    RB_TRY(to_dev(&d_off, cv_off.data(), nc, c->stream));
-    RB_TRY(to_dev(&d_init, p->init_counts, M1, c->stream));
-    RB_TRY(to_dev(&d_alpha, p->pseudo_counts, M1, c->stream));
-    RB_TRY(to_dev(&d_eel, p->eel, M1, c->stream));
-    RB_TRY(to_dev(&d_mw, p->mw, M1, c->stream));
-    RB_TRY(to_dev(&d_gene, p->gene_start, (size_t)p->n_genes + 1, c->stream));
-    RB_TRYC(cudaMalloc(&d_counts, (size_t)nc * M1 * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_counts0, (size_t)nc * M1 * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_z, (size_t)nc * 2 * g.N1 * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_u, (size_t)nc * 2 * g.N1 * sizeof(unsigned)));
-    RB_TRYC(cudaMalloc(&d_flips, (size_t)nc * 4 * W * sizeof(unsigned)));
-    RB_TRYC(cudaMalloc(&d_pre, (size_t)nc * W * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_tot, (size_t)nc * ctas * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_sync, (size_t)nc * sizeof(ChainSync)));
-    RB_TRYC(cudaMalloc(&d_cv, std::max<size_t>((size_t)total_samples * M1, 1) * sizeof(int)));
-    RB_TRYC(cudaMalloc(&d_acc, (size_t)nc * acc_per * sizeof(double)));
-    RB_TRYC(cudaMalloc(&d_tmp, (size_t)nc * 2 * M1 * sizeof(double)));
-    RB_TRYC(cudaMemsetAsync(d_acc, 0, (size_t)nc * acc_per * sizeof(double), c->stream));
-    RB_TRYC(cudaMemsetAsync(d_sync, 0, (size_t)nc * sizeof(ChainSync), c->stream));
-    RB_TRYC(cudaMemsetAsync(d_tot, 0, (size_t)nc * ctas * sizeof(int), c->stream));
-    a.chain_samples = d_samples; a.chain_seeds = d_seeds; a.chain_cv_offset = d_off; a.init_counts = d_init;
-    a.alpha = d_alpha; a.eel = d_eel; a.mw = d_mw; a.gene_start = d_gene; a.counts = d_counts; a.counts_start = d_counts0; a.z = d_z;
-    a.ubuf = d_u; a.flips = d_flips; a.pre = d_pre; a.slice_tot = d_tot; a.sync = d_sync; a.count_vectors = d_cv; a.acc = d_acc;
-    a.theta_tmp = d_tmp;
+    const GParts q = gparts(g.N1, g.E, p->M, false, p->n_genes, n_samples, nc, ctas);
+    const Scratch s = scratch_parts((size_t)p->M + 1, g.N1, nc, 0);
+    RunBlock run;
+    if (int rc = upload_run(c, p, q, s.total, run)) return rc;
+    unsigned char* sb = run.p + q.run;
 
+    PArgs a{};
+    static_cast<RunArgs&>(a) = run_args(run.p, q, p, reinterpret_cast<double*>(sb + s.theta));
+    set_layout(a, g.v, g.N1, g.n_segs);
+    a.n_chains = nc;
+    a.counts = reinterpret_cast<int*>(sb + s.counts);
+    a.counts_start = reinterpret_cast<int*>(sb + s.counts_start);
+    a.z = reinterpret_cast<int*>(sb + s.z);
+    a.ubuf = reinterpret_cast<unsigned*>(sb + s.ubuf);
+    a.flips = reinterpret_cast<unsigned*>(sb + s.flips);
+    a.pre = reinterpret_cast<int*>(sb + s.pre);
+    a.slice_tot = reinterpret_cast<int*>(run.p + q.slice_tot);
     {
         const char* e = getenv("RSEM_B200_GIBBS_FAST");
         a.fast_rows = !(e && !strcmp(e, "0"));
@@ -1529,19 +1617,13 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
         a.chain_base = base;
         a.ctas_per_chain = ctas;
         void* kargs[] = {(void*)&a};
-        RB_TRYC(cudaLaunchCooperativeKernel(kernel, dim3(wave * (ctas + 1)), dim3(kPThreads), kargs, 0, c->stream));
+        RB_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(wave * (ctas + 1)), dim3(kPThreads), kargs, 0, c->stream));
         c->launches++;
         ++waves;
     }
     if (timing || stats) cudaEventRecord(ev1, c->stream);
     std::vector<ChainSync> h_sync(nc);
-    RB_TRYC(cudaMemcpyAsync(chain_acc, d_acc, (size_t)nc * acc_per * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaMemcpyAsync(count_vectors, d_cv, (size_t)total_samples * M1 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaMemcpyAsync(h_sync.data(), d_sync, (size_t)nc * sizeof(ChainSync), cudaMemcpyDeviceToHost, c->stream));
-    RB_TRYC(cudaStreamSynchronize(c->stream));
-    cleanup();
-#undef RB_TRY
-#undef RB_TRYC
+    const int rc = read_run(c, run.p, q, nc, n_samples, p->M, p->n_genes, count_vectors, chain_acc, h_sync.data());
     if (timing || stats) {
         float ms = 0;
         cudaEventElapsedTime(&ms, ev0, ev1);
@@ -1557,68 +1639,18 @@ static int gibbs_run_parallel(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p,
         fprintf(stderr, "gibbs chain 0 (%d worker CTAs, %d segments): %u passes; worker CTA 0 thread 0 cycles: wait for uniforms %llu, passes %llu, "
                 "barriers + bookkeeping %llu (incl. the passes), per-sample work %llu\n", ctas, g.n_segs, h_sync[0].passes, h_sync[0].prof[0],
                 h_sync[0].prof[1], h_sync[0].prof[2], h_sync[0].prof[3]);
-    for (int t = 0; t < nc; ++t)
-        if (h_sync[t].err) {
-            set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
-            return RSEM_B200_ERR_ARG;
-        }
-    return 0;
+    return rc;
 }
 
 int gibbs_run(rsem_b200_ctx* c, const rsem_b200_gibbs_params* p, int32_t* count_vectors, double* chain_acc,
               rsem_b200_gibbs_stats* stats) {
-    // a row without entries has nothing to draw from (both kernels would fall off its empty cumulative array)
-    if (c->gibbs.empty_row) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
+    if (c->gibbs.empty_row) return refuse_empty_row();
     const char* mode = getenv("RSEM_B200_GIBBS");   // "serial" = the one-warp-per-chain kernel (cross-check / debugging)
     if (mode && !strcmp(mode, "serial")) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
     // tiny inputs: a 624-word regeneration would span more than two sweeps (the generator runs only one sweep ahead)
-    if (c->gibbs.N1 < 1248 || !c->gibbs.order) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
+    if (c->gibbs.N1 < 1248) return gibbs_run_serial(c, p, count_vectors, chain_acc, stats);
     return gibbs_run_parallel(c, p, count_vectors, chain_acc, stats);
 }
-
-// ---- K13 host side ------------------------------------------------------------------------------------------------------
-namespace {
-constexpr int kBatchMaxWorkers = 8;   // worker CTAs per team; slice totals are sized for it
-constexpr int kBatchDefaultWorkers = 2;
-
-size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// byte offsets of a sample's parts in its block; n_segs <= N1 and comp_tids <= M + 1 bound the layout before it is built
-struct GParts {
-    size_t order, p_off, p_sid, p_con, seg_start, seg_ntr, seg_tid_off, comp_tids, init, alpha, eel, mw, gene, samples, seeds,
-        cv_off, head, sync, slice_tot, acc, zero_end, cv, total;
-};
-GParts gparts(uint64_t N1, uint64_t E, int M, int n_genes, int n_samples, int n_chains) {
-    const size_t M1 = (size_t)M + 1;
-    GParts p{};
-    size_t at = 0;
-    auto put = [&](size_t& off, size_t bytes) { off = at; at = align_up(at + bytes); };
-    put(p.order, N1 * 4);
-    put(p.p_off, (N1 + 1) * 8);
-    put(p.p_sid, (E + 16) * 4);
-    put(p.p_con, (E + 16) * 8);
-    put(p.seg_start, (N1 + 1) * 4);
-    put(p.seg_ntr, std::max<uint64_t>(N1, 1) * 4);
-    put(p.seg_tid_off, (N1 + 1) * 4);
-    put(p.comp_tids, (M1 + 1) * 4);
-    put(p.init, M1 * 4);
-    put(p.alpha, M1 * 8);
-    put(p.eel, M1 * 8);
-    put(p.mw, M1 * 8);
-    put(p.gene, ((size_t)n_genes + 1) * 4);
-    put(p.samples, (size_t)n_chains * 4);
-    put(p.seeds, (size_t)n_chains * 4);
-    put(p.cv_off, (size_t)n_chains * 8);
-    p.head = at;
-    put(p.sync, (size_t)n_chains * sizeof(ChainSync));
-    put(p.slice_tot, (size_t)n_chains * kBatchMaxWorkers * 4);
-    put(p.acc, (size_t)n_chains * (4 * M1 + (size_t)n_genes) * 8);
-    p.zero_end = at;
-    put(p.cv, (size_t)n_samples * M1 * 4);
-    p.total = at;
-    return p;
-}
-}  // namespace
 
 }  // namespace rsem_b200
 
@@ -1631,7 +1663,7 @@ struct rsem_b200_gibbs_batch {
         uint64_t cost = 0;                 // reads x sweeps of its longest chain: the claim order
         std::vector<int32_t> chain_samples;
         rsem_b200::PArgs a{};              // device pointers into the block; scratch pointers are the team's
-        size_t sync_off = 0, acc_off = 0, cv_off = 0;
+        rsem_b200::GParts q{};             // the block: layout part, then the run part at q.layout
     };
     rsem_b200_ctx* ctx = nullptr;
     uint64_t capacity = 0, used = 0;
@@ -1673,6 +1705,7 @@ void gibbs_batch_destroy(rsem_b200_gibbs_batch* b) {
     delete b;
 }
 
+
 int gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes, int32_t n_samples, int32_t n_chains,
                              uint64_t* bytes) {
     if (N1 < RSEM_B200_GIBBS_BATCH_MIN_READS || N1 > RSEM_B200_GIBBS_BATCH_MAX_READS) {
@@ -1680,7 +1713,8 @@ int gibbs_batch_sample_bytes(uint64_t N1, uint64_t E, int32_t M, int32_t n_genes
                   "rsem_b200_gibbs_upload + rsem_b200_gibbs_run_chains");
         return RSEM_B200_ERR_UNSUPPORTED;
     }
-    *bytes = gparts(N1, E, M, n_genes, n_samples, n_chains).total;
+    const GParts q = gparts(N1, E, M, false, n_genes, n_samples, n_chains, kBatchMaxWorkers);
+    *bytes = q.layout + q.run;
     return 0;
 }
 
@@ -1707,43 +1741,21 @@ int gibbs_batch_add(rsem_b200_gibbs_batch* b, uint64_t N1, uint64_t E, const uin
     }
     GibbsLayout L;
     if (int rc = gibbs_layout(row_ptr, sid, N1, M, L)) return rc;
-    // a row without entries has nothing to draw from (as gibbs_run refuses it)
-    if (L.empty_row) { set_error("gibbs: a read without any entry (the .ofg writer never emits one)"); return RSEM_B200_ERR_ARG; }
-    const GParts q = gparts(N1, E, M, p->n_genes, (int)n_samples, nc);
-    const size_t M1 = (size_t)M + 1;
-    std::vector<unsigned char> img(q.head, 0);
-    auto put = [&](size_t off, const void* src, size_t n) { if (n) memcpy(img.data() + off, src, n); };
-    put(q.order, L.order.data(), N1 * 4);
-    put(q.p_off, L.p_off.data(), (N1 + 1) * 8);
-    put(q.p_sid, L.p_sid.data(), E * 4);
-    {
-        double* pc = reinterpret_cast<double*>(img.data() + q.p_con);
-        for (uint64_t r = 0; r < N1; ++r) {
-            const uint64_t src = row_ptr[L.order[r]], n = row_ptr[L.order[r] + 1] - src;
-            memcpy(pc + L.p_off[r], conprb + src, n * 8);
-        }
+    if (L.empty_row) return refuse_empty_row();
+    const GParts q = gparts(N1, E, M, false, p->n_genes, n_samples, nc, kBatchMaxWorkers);
+    std::vector<unsigned char> img(q.layout + q.zero, 0);
+    pack_layout([&](size_t off, const void* src, size_t n) { put(img.data(), off, src, n); }, q, L);
+    for (uint64_t r = 0; r < N1; ++r) {   // conprb in slot order
+        const uint64_t src = row_ptr[L.order[r]], n = row_ptr[L.order[r] + 1] - src;
+        put(img.data(), q.p_con + L.p_off[r] * 8, conprb + src, n * 8);
     }
-    put(q.seg_start, L.seg_start.data(), L.seg_start.size() * 4);
-    put(q.seg_ntr, L.seg_ntr.data(), L.seg_ntr.size() * 4);
-    put(q.seg_tid_off, L.seg_tid_off.data(), L.seg_tid_off.size() * 4);
-    put(q.comp_tids, L.comp_tids.data(), L.comp_tids.size() * 4);
-    put(q.init, p->init_counts, M1 * 4);
-    put(q.alpha, p->pseudo_counts, M1 * 8);
-    put(q.eel, p->eel, M1 * 8);
-    put(q.mw, p->mw, M1 * 8);
-    put(q.gene, p->gene_start, ((size_t)p->n_genes + 1) * 4);
-    put(q.samples, p->chain_samples, (size_t)nc * 4);
-    put(q.seeds, p->chain_seeds, (size_t)nc * 4);
-    {
-        long long* off = reinterpret_cast<long long*>(img.data() + q.cv_off);
-        long long at = 0;
-        for (int t = 0; t < nc; ++t) { off[t] = at; at += p->chain_samples[t]; }
-    }
+    pack_run(img.data() + q.layout, q, p);
     RB_CUDA(cudaSetDevice(c->device));
     void* block = nullptr;
-    RB_CUDA(cudaMallocAsync(&block, q.total, c->stream));
-    RB_CUDA(cudaMemcpyAsync(block, img.data(), q.head, cudaMemcpyHostToDevice, c->stream));
-    RB_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(block) + q.head, 0, q.zero_end - q.head, c->stream));   // sync, slice totals, sums
+    RB_CUDA(cudaMallocAsync(&block, bytes, c->stream));
+    unsigned char* base = static_cast<unsigned char*>(block);
+    RB_CUDA(cudaMemcpyAsync(base, img.data(), img.size(), cudaMemcpyHostToDevice, c->stream));
+    RB_CUDA(cudaMemsetAsync(base + q.layout + q.zero, 0, q.cv - q.zero, c->stream));   // chain states, slice totals, sums
     RB_CUDA(cudaStreamSynchronize(c->stream));   // img goes out of scope
 
     int slot = -1;
@@ -1758,36 +1770,14 @@ int gibbs_batch_add(rsem_b200_gibbs_batch* b, uint64_t N1, uint64_t E, const uin
     s.n_samples = (int)n_samples;
     s.cost = longest * N1;
     s.chain_samples.assign(p->chain_samples, p->chain_samples + nc);
-    s.sync_off = q.sync; s.acc_off = q.acc; s.cv_off = q.cv;
-    unsigned char* base = static_cast<unsigned char*>(block);
+    s.q = q;
     PArgs& a = s.a;
-    a.N1 = N1;
-    a.order = reinterpret_cast<const int*>(base + q.order);
-    a.p_off = reinterpret_cast<const unsigned long long*>(base + q.p_off);
-    a.p_sid = reinterpret_cast<const int*>(base + q.p_sid);
-    a.p_con = reinterpret_cast<const double*>(base + q.p_con);
-    a.seg_start = reinterpret_cast<const int*>(base + q.seg_start);
-    a.seg_ntr = reinterpret_cast<const int*>(base + q.seg_ntr);
-    a.seg_tid_off = reinterpret_cast<const int*>(base + q.seg_tid_off);
-    a.comp_tids = reinterpret_cast<const int*>(base + q.comp_tids);
-    a.n_segs = L.n_segs;
+    static_cast<RunArgs&>(a) = run_args(base + q.layout, q, p, nullptr);
+    set_layout(a, layout_view(base, q), N1, L.n_segs);
     a.fast_rows = 1;
-    a.M = M; a.burnin = p->burnin; a.gap = p->gap; a.n_genes = p->n_genes; a.n_chains = nc;
+    a.n_chains = nc;
     a.ctas_per_chain = b->k;
-    a.chain_samples = reinterpret_cast<const int*>(base + q.samples);
-    a.chain_seeds = reinterpret_cast<const unsigned*>(base + q.seeds);
-    a.chain_cv_offset = reinterpret_cast<const long long*>(base + q.cv_off);
-    a.n0 = p->n0; a.totc = p->totc;
-    a.init_counts = reinterpret_cast<const int*>(base + q.init);
-    a.alpha = reinterpret_cast<const double*>(base + q.alpha);
-    a.eel = reinterpret_cast<const double*>(base + q.eel);
-    a.mw = reinterpret_cast<const double*>(base + q.mw);
-    a.gene_start = reinterpret_cast<const int*>(base + q.gene);
-    a.slice_tot = reinterpret_cast<int*>(base + q.slice_tot);
-    a.n_words = (unsigned)((N1 + 31) / 32);
-    a.sync = reinterpret_cast<ChainSync*>(base + q.sync);
-    a.count_vectors = reinterpret_cast<int*>(base + q.cv);
-    a.acc = reinterpret_cast<double*>(base + q.acc);
+    a.slice_tot = reinterpret_cast<int*>(base + q.layout + q.slice_tot);
     b->used += bytes;
     b->M = M;
     b->n_genes = p->n_genes;
@@ -1824,30 +1814,26 @@ int gibbs_batch_run(rsem_b200_gibbs_batch* b, rsem_b200_gibbs_batch_stats* stats
     if (resident < b->k + 1) { set_error("gibbs_batch_run: a team does not fit the device"); return RSEM_B200_ERR_UNSUPPORTED; }
     const int teams = std::min<int>((int)jobs.size(), resident / (b->k + 1));
     const int M1 = b->M + 1;
-    const unsigned w_max = (unsigned)((n1_max + 31) / 32);
 
     BArgs ba{};
     ba.n_jobs = (unsigned)jobs.size();
     ba.k = (unsigned)b->k;
     ba.n1_max = n1_max;
-    ba.w_max = w_max;
+    ba.w_max = (unsigned)((n1_max + 31) / 32);
     ba.M1 = M1;
     void* scratch = nullptr;
-    const size_t per_team[] = {(size_t)M1 * 4, (size_t)M1 * 4, 2 * n1_max * 4, 2 * n1_max * 4, 4 * (size_t)w_max * 4,
-                               (size_t)w_max * 4, 2 * (size_t)M1 * 8};
-    size_t off[8] = {0};
-    for (int i = 0; i < 7; ++i) off[i + 1] = off[i] + align_up(per_team[i] * teams);
+    const Scratch st = scratch_parts(M1, n1_max, teams, 0);
     const size_t head = align_up(args.size() * sizeof(PArgs)) + align_up(jobs.size() * sizeof(int2)) + 256 + align_up(teams * 8ull);
-    RB_CUDA(cudaMallocAsync(&scratch, off[7] + head, c->stream));
+    RB_CUDA(cudaMallocAsync(&scratch, st.total + head, c->stream));
     unsigned char* sb = static_cast<unsigned char*>(scratch);
-    ba.counts = reinterpret_cast<int*>(sb + off[0]);
-    ba.counts_start = reinterpret_cast<int*>(sb + off[1]);
-    ba.z = reinterpret_cast<int*>(sb + off[2]);
-    ba.ubuf = reinterpret_cast<unsigned*>(sb + off[3]);
-    ba.flips = reinterpret_cast<unsigned*>(sb + off[4]);
-    ba.pre = reinterpret_cast<int*>(sb + off[5]);
-    ba.theta_tmp = reinterpret_cast<double*>(sb + off[6]);
-    unsigned char* hp = sb + off[7];
+    ba.counts = reinterpret_cast<int*>(sb + st.counts);
+    ba.counts_start = reinterpret_cast<int*>(sb + st.counts_start);
+    ba.z = reinterpret_cast<int*>(sb + st.z);
+    ba.ubuf = reinterpret_cast<unsigned*>(sb + st.ubuf);
+    ba.flips = reinterpret_cast<unsigned*>(sb + st.flips);
+    ba.pre = reinterpret_cast<int*>(sb + st.pre);
+    ba.theta_tmp = reinterpret_cast<double*>(sb + st.theta);
+    unsigned char* hp = sb + st.total;
     ba.samples = reinterpret_cast<const PArgs*>(hp);
     hp += align_up(args.size() * sizeof(PArgs));
     ba.jobs = reinterpret_cast<const int2*>(hp);
@@ -1880,40 +1866,32 @@ int gibbs_batch_run(rsem_b200_gibbs_batch* b, rsem_b200_gibbs_batch_stats* stats
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (rc) return rc;
-    bool err = false;
+    int err = 0;
     uint64_t chain_cyc = 0, sample_cyc = 0;
     for (int i : run) {
         auto& s = b->slots[i];
         std::vector<ChainSync> sy(s.n_chains);
-        RB_CUDA(cudaMemcpy(sy.data(), static_cast<unsigned char*>(s.block) + s.sync_off, s.n_chains * sizeof(ChainSync),
-                           cudaMemcpyDeviceToHost));
+        const int r = read_run(c, static_cast<unsigned char*>(s.block) + s.q.layout, s.q, s.n_chains, s.n_samples, b->M, b->n_genes,
+                               nullptr, nullptr, sy.data());
+        if (r && r != RSEM_B200_ERR_ARG) return r;   // RSEM_B200_ERR_ARG: a draw fell off, reported after the stats
+        err = err ? err : r;
         for (const ChainSync& y : sy) {
-            err = err || y.err;
             chain_cyc += y.prof[0] + y.prof[2] + y.prof[3];
             sample_cyc += y.prof[3];
         }
         s.ran = true;
     }
     if (stats) *stats = rsem_b200_gibbs_batch_stats{ms, b->k, teams, (int64_t)jobs.size(), chain_cyc, sample_cyc};
-    if (err) {
-        set_error("gibbs: categorical draw fell off the cumulative array (reference: assert(l < len), sampling.h:62)");
-        return RSEM_B200_ERR_ARG;
-    }
-    return 0;
+    return err;
 }
 
 int gibbs_batch_result(rsem_b200_gibbs_batch* b, int32_t slot, int32_t* count_vectors, double* chain_acc) {
     if (slot < 0 || slot >= (int)b->slots.size() || !b->slots[slot].live) { set_error("no sample in this slot"); return RSEM_B200_ERR_ARG; }
     const auto& s = b->slots[slot];
     if (!s.ran) { set_error("gibbs_batch_result: the sample has not run yet"); return RSEM_B200_ERR_ARG; }
-    rsem_b200_ctx* c = b->ctx;
-    const size_t M1 = (size_t)b->M + 1, acc_per = 4 * M1 + (size_t)b->n_genes;
-    RB_CUDA(cudaSetDevice(c->device));
-    const unsigned char* base = static_cast<const unsigned char*>(s.block);
-    RB_CUDA(cudaMemcpyAsync(count_vectors, base + s.cv_off, (size_t)s.n_samples * M1 * 4, cudaMemcpyDeviceToHost, c->stream));
-    RB_CUDA(cudaMemcpyAsync(chain_acc, base + s.acc_off, (size_t)s.n_chains * acc_per * 8, cudaMemcpyDeviceToHost, c->stream));
-    RB_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    RB_CUDA(cudaSetDevice(b->ctx->device));
+    return read_run(b->ctx, static_cast<unsigned char*>(s.block) + s.q.layout, s.q, s.n_chains, s.n_samples, b->M, b->n_genes,
+                    count_vectors, chain_acc, nullptr);
 }
 
 }  // namespace rsem_b200
