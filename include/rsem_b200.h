@@ -317,7 +317,8 @@ typedef struct rsem_b200_sim_stats rsem_b200_sim_stats;
  *   profile_cdf     pro_rows x 5 x 5: QProfile (100 rows, QProfile.h:151-193) or Profile (proLen rows,
  *                   Profile.h:163-205), after the reference's zero-row repair
  *   noise_cdf       NoiseQProfile 100 x 5 (NoiseQProfile.h:153-166) or NoiseProfile 5 (NoiseProfile.h:137-144)
- *   seq / seq_off   forward-strand base codes 0..4 (A C G T N) per transcript, as upload_refs takes them
+ *   seq / seq_off   forward-strand base codes 0..4 (A C G T N) per transcript, as upload_refs takes them; seq ==
+ *                   NULL: the reference of rsem_b200_sim_upload_refs (seq_off, tot_len and full_len are then not read)
  * exact_body = 1 when a reachable table row sums to 0 (simul.h:29-32 then draws a second word), so the number of
  * words an attempt takes depends on the drawn qualities.  With 0 the attempt lengths are computed from the first
  * draws only; a wrong 0 gives wrong reads.
@@ -348,7 +349,14 @@ typedef struct rsem_b200_sim_params {
     const int32_t* full_len;   /* M + 1 */
 } rsem_b200_sim_params;
 
-/* uploads the tables and seeds the stream (simulation.cpp:117-120, simul.h:11) */
+/* Keeps a reference on the context for the runs that follow: rsem_b200_sim_begin with params->seq == NULL uses it
+ * (its M must be params->M) instead of uploading the params' own.  Replaces an earlier upload; freed with the context.
+ * Not while a run is between sim_begin and sim_end.                                                          */
+int rsem_b200_sim_upload_refs(rsem_b200_ctx* ctx, int32_t M, const uint64_t* seq_off, const uint8_t* seq,
+                              const int32_t* tot_len, const int32_t* full_len);
+/* uploads the tables and seeds the stream (simulation.cpp:117-120, simul.h:11).  The device buffers of a run stay on
+ * the context after sim_end and are reused by its next run (grown when that run needs more), so a context that runs
+ * sample after sample allocates nothing after its largest one; rsem_b200_ctx_destroy frees them.              */
 int rsem_b200_sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* params);
 /* the next chunk of reads, in order (simulation.cpp:121-126): *n_reads reads as the text of the read file(s)
  * (SingleRead(Q)::write, PairedEndRead(Q)::write: mate 1 in text[0], mate 2 in text[1]).  The buffers belong to the
@@ -365,7 +373,7 @@ typedef struct rsem_b200_sim_stats {
     uint64_t windows;
 } rsem_b200_sim_stats;
 /* counts[sid] of the simulated reads (M + 1), the number of failed attempts ("resimulation") and, when stats is not
- * NULL, the phase times; frees the state                                                                     */
+ * NULL, the phase times; ends the run (its buffers stay on the context)                                      */
 int rsem_b200_sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 
 /* ---- read simulation over several contexts (RSEM_B200_DEVICES) ----------------------------------------------------
@@ -387,7 +395,7 @@ typedef struct rsem_b200_sim_devices_stats {
                                  window's entry point                                                         */
 } rsem_b200_sim_devices_stats;
 /* counts and failed attempts summed over the contexts, stats (may be NULL), per_device (n entries, may be NULL: each
- * context's own phases); frees every context's simulation state and the handle                             */
+ * context's own phases); ends every context's run and frees the handle                                     */
 int rsem_b200_sim_end_devices(rsem_b200_sim_multi* multi, double* counts, uint64_t* resim,
                               rsem_b200_sim_devices_stats* stats, rsem_b200_sim_stats* per_device);
 /* Device-free: state_out = the boost::mt19937 state after J draws from state_in.  state[0..623] are the words,

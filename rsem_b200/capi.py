@@ -151,6 +151,7 @@ SYMBOLS = [
     "rsem_b200_gibbs_batch_destroy", "rsem_b200_gibbs_batch_sample_bytes", "rsem_b200_gibbs_batch_add",
     "rsem_b200_gibbs_batch_run", "rsem_b200_gibbs_batch_result", "rsem_b200_gibbs_batch_clear",
     "rsem_b200_sim_begin_devices", "rsem_b200_sim_next_devices", "rsem_b200_sim_end_devices", "rsem_b200_mt19937_jump",
+    "rsem_b200_sim_upload_refs",
 ]
 
 RSEM_B200_ERR_ARG = 2
@@ -382,6 +383,15 @@ class Context:
     def gibbs_upload_from(self, src: "Context"):
         """this context gets the matrix uploaded to src (device-to-device copies)"""
         self.lib.check(self.lib.dll.rsem_b200_gibbs_upload_from(self._h, src._h if src is not None else None))
+
+    def sim_upload_refs(self, seq_off: np.ndarray, seq: np.ndarray, tot_len: np.ndarray, full_len: np.ndarray):
+        """keeps the reference on the context (M = len(tot_len) - 1): a following sim_begin whose params.seq is NULL
+        uses it"""
+        seq_off, seq = _arr(seq_off, np.uint64), _arr(seq, np.uint8)
+        tot_len, full_len = _arr(tot_len, np.int32), _arr(full_len, np.int32)
+        self.lib.check(self.lib.dll.rsem_b200_sim_upload_refs(self._h, C.c_int32(len(tot_len) - 1), _p(seq_off, C.c_uint64),
+                                                              _p(seq, C.c_uint8), _p(tot_len, C.c_int32),
+                                                              _p(full_len, C.c_int32)))
 
     def sim_begin(self, params: SimParams):
         """params' arrays must stay alive until sim_begin returns (they are copied to the device)"""

@@ -865,8 +865,8 @@ int rsem_b200_gibbs_batch_clear(rsem_b200_gibbs_batch* b) {
 namespace {
 int check_sim_params(const rsem_b200_sim_params* p) {
     RB_ARG(p->model_type >= 0 && p->model_type <= 3 && p->M >= 1, "bad model type or M");
-    RB_ARG(p->theta_cdf && p->gld.cdf && p->profile_cdf && p->noise_cdf && p->seq_off && p->seq && p->tot_len &&
-               p->full_len, "NULL table");
+    RB_ARG(p->theta_cdf && p->gld.cdf && p->profile_cdf && p->noise_cdf, "NULL table");
+    RB_ARG(!p->seq || (p->seq_off && p->tot_len && p->full_len), "NULL reference table");
     RB_ARG(p->gld.span == p->gld.ub - p->gld.lb && p->gld.span >= 1, "bad gld");
     RB_ARG(p->model_type < 2 || p->has_mld, "paired-end models need mld");
     RB_ARG(!p->has_mld || (p->mld.cdf && p->mld.span == p->mld.ub - p->mld.lb && p->mld.span >= 1), "bad mld");
@@ -881,6 +881,14 @@ int rsem_b200_sim_begin(rsem_b200_ctx* c, const rsem_b200_sim_params* p) {
     if (int rc = check_sim_params(p)) return rc;
     RB_CUDA(cudaSetDevice(c->device));
     return sim_begin(c, p);
+}
+
+int rsem_b200_sim_upload_refs(rsem_b200_ctx* c, int32_t M, const uint64_t* seq_off, const uint8_t* seq,
+                              const int32_t* tot_len, const int32_t* full_len) {
+    RB_ARG(c && seq_off && seq && tot_len && full_len, "NULL argument");
+    RB_ARG(M >= 1, "bad M");
+    RB_CUDA(cudaSetDevice(c->device));
+    return sim_upload_refs(c, M, seq_off, seq, tot_len, full_len);
 }
 
 int rsem_b200_sim_next(rsem_b200_ctx* c, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {

@@ -279,7 +279,7 @@ struct rsem_b200_ctx {
     rsem_b200::DevRefs refs;
 
     rsem_b200::DevGibbs gibbs;
-    rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads between sim_begin and sim_end
+    rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads: the run, its kept buffers and the uploaded reference
     rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals between ci_begin and ci_end
     rsem_b200::GbamState* gbam = nullptr;  // rsem-tbam2gbam: transcript tables and batch scratch
     rsem_b200::WigState* wig = nullptr;    // rsem-bam2wig / rsem-bam2readdepth: the resident run and batch scratch
@@ -397,6 +397,8 @@ int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p);
 int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
 int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats);
 void sim_free(rsem_b200_ctx* ctx);
+int sim_upload_refs(rsem_b200_ctx* ctx, int M, const uint64_t* seq_off, const uint8_t* seq, const int32_t* tot_len,
+                    const int32_t* full_len);
 int sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_params* p, rsem_b200_sim_multi** out);
 int sim_next_devices(rsem_b200_sim_multi* m, const char* text[2], uint64_t bytes[2], uint64_t* n_reads);
 int sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rsem_b200_sim_devices_stats* stats,

@@ -29,6 +29,7 @@
 #include <chrono>
 #include <cstring>
 #include <memory>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -456,29 +457,27 @@ __global__ void sim_write_kernel(SimTables t, const uint32_t* __restrict__ words
     atomicAdd(counts + h.sid, 1.0);
 }
 
-template <class T>
-T* dev_copy(const T* src, size_t n, std::vector<void*>& owned) {
-    T* d = nullptr;
-    if (cudaMalloc(&d, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return nullptr;
-    owned.push_back(d);
-    if (n && cudaMemcpy(d, src, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-    return d;
-}
-
 }  // namespace
 
+// The state of the context's runs.  A run (sim_begin .. sim_end) fills the fields from `t` to `jump_ms`; the device
+// buffers, the generator stream, the events and the host text buffers are kept from run to run and freed by sim_free
+// (rsem_b200_ctx_destroy), so that a context running sample after sample (rsem-simulate-reads-batch) makes no
+// cudaMalloc / cudaFree call, each of which synchronises the whole device, unless a run needs more than the runs before.
 struct SimState {
+    bool running = false;          // between sim_begin and sim_end
     SimTables t{};
     bool exact_body = false;
     uint64_t N = 0, done = 0, resim = 0;
     uint32_t W = 0, L = 0, K = 0;
     uint32_t entry = 0;
     uint64_t window = 0;           // index of the window sim_next processes next
-    std::vector<void*> owned;
     cudaStream_t gen_stream = nullptr;  // the generator runs one window ahead on its own stream
     cudaEvent_t gen_ev[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // per buffer: generation start / end
     cudaEvent_t used_ev[2] = {nullptr, nullptr};                           // per buffer: its window is resolved and read
     cudaEvent_t ph_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // the run's buffers, carved out of `arena` (sim_layout)
+    char* arena = nullptr;
+    size_t arena_bytes = 0;
     uint32_t* mt = nullptr;          // 625 words
     uint32_t* words[2] = {nullptr, nullptr};  // W + L each
     uint32_t* len = nullptr;         // W
@@ -495,11 +494,18 @@ struct SimState {
     void* scan_tmp = nullptr;
     size_t scan_tmp_bytes = 0;
     char* text_d[2] = {nullptr, nullptr};
-    size_t text_cap = 0;
+    size_t text_cap[2] = {0, 0};
     std::vector<char> text_h[2][2];  // [slot][mate]: a chunk stays valid until the second following sim_next
     int slot = 0;
     double* counts = nullptr;
     rsem_b200_sim_stats stats{};
+    // the reference of rsem_b200_sim_upload_refs, used by runs whose params carry no sequences
+    int ref_M = 0;
+    void* ref_block = nullptr;
+    const uint64_t* ref_seq_off = nullptr;
+    const uint8_t* ref_seq = nullptr;
+    const int32_t* ref_tot_len = nullptr;
+    const int32_t* ref_full_len = nullptr;
 
     // one of G >= 2 contexts of sim_begin_devices: `window` counts this context's own windows, each W + L fresh words
     // followed by a jump to the start of its next one
@@ -519,7 +525,8 @@ void sim_free(rsem_b200_ctx* ctx) {
     if (!s) return;
     cudaStreamSynchronize(ctx->stream);
     if (s->gen_stream) cudaStreamSynchronize(s->gen_stream);
-    for (void* p : s->owned) cudaFree(p);
+    cudaFree(s->arena);
+    cudaFree(s->ref_block);
     cudaFree(s->text_d[0]);
     cudaFree(s->text_d[1]);
     for (auto& e : s->gen_ev) for (cudaEvent_t x : e) if (x) cudaEventDestroy(x);
@@ -532,11 +539,64 @@ void sim_free(rsem_b200_ctx* ctx) {
     ctx->sim = nullptr;
 }
 
-#define SIM_ALLOC(ptr, n)                                                       \
-    do {                                                                        \
-        RB_CUDA(cudaMalloc(&(ptr), std::max<size_t>((n), 1) * sizeof(*(ptr)))); \
-        s->owned.push_back((void*)(ptr));                                       \
-    } while (0)
+namespace {
+
+// the context's SimState with its generator stream and events, created on first use
+int sim_state(rsem_b200_ctx* ctx, SimState** out) {
+    if (!ctx->sim) {
+        SimState* s = new SimState();
+        ctx->sim = s;
+        auto make = [&]() -> int {
+            RB_CUDA(cudaStreamCreateWithFlags(&s->gen_stream, cudaStreamNonBlocking));
+            for (auto& e : s->gen_ev) for (cudaEvent_t& x : e) RB_CUDA(cudaEventCreate(&x));
+            for (cudaEvent_t& x : s->used_ev) RB_CUDA(cudaEventCreate(&x));
+            for (cudaEvent_t& x : s->ph_ev) RB_CUDA(cudaEventCreate(&x));
+            for (cudaEvent_t& x : s->jump_ev) RB_CUDA(cudaEventCreate(&x));
+            for (auto& e : s->prep_ev) for (cudaEvent_t& x : e) RB_CUDA(cudaEventCreate(&x));
+            return 0;
+        };
+        if (int rc = make()) { sim_free(ctx); return rc; }
+    }
+    *out = ctx->sim;
+    return 0;
+}
+
+// a run's end: nothing of it is left on either stream, its buffers stay for the next run
+void sim_stop(rsem_b200_ctx* ctx) {
+    SimState* s = ctx->sim;
+    if (!s || !s->running) return;
+    cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(s->gen_stream);
+    s->running = false;
+}
+
+}  // namespace
+
+int sim_upload_refs(rsem_b200_ctx* ctx, int M, const uint64_t* seq_off, const uint8_t* seq, const int32_t* tot_len,
+                    const int32_t* full_len) {
+    SimState* s = nullptr;
+    if (int rc = sim_state(ctx, &s)) return rc;
+    RB_ARG(!s->running, "sim_upload_refs: a simulation is running on this context (rsem_b200_sim_end first)");
+    cudaFree(s->ref_block);
+    s->ref_block = nullptr;
+    s->ref_M = 0;
+    const size_t n_off = ((size_t)M + 2) * sizeof(uint64_t), n_len = ((size_t)M + 1) * sizeof(int32_t);
+    const size_t n_seq = seq_off[M + 1];
+    char* b = nullptr;
+    RB_CUDA(cudaMalloc(&b, n_off + 2 * n_len + n_seq + 1));
+    s->ref_block = b;
+    RB_CUDA(cudaMemcpyAsync(b, seq_off, n_off, cudaMemcpyHostToDevice, ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(b + n_off, tot_len, n_len, cudaMemcpyHostToDevice, ctx->stream));
+    RB_CUDA(cudaMemcpyAsync(b + n_off + n_len, full_len, n_len, cudaMemcpyHostToDevice, ctx->stream));
+    if (n_seq) RB_CUDA(cudaMemcpyAsync(b + n_off + 2 * n_len, seq, n_seq, cudaMemcpyHostToDevice, ctx->stream));
+    RB_CUDA(cudaStreamSynchronize(ctx->stream));
+    s->ref_seq_off = reinterpret_cast<const uint64_t*>(b);
+    s->ref_tot_len = reinterpret_cast<const int32_t*>(b + n_off);
+    s->ref_full_len = reinterpret_cast<const int32_t*>(b + n_off + n_len);
+    s->ref_seq = reinterpret_cast<const uint8_t*>(b + n_off + 2 * n_len);
+    s->ref_M = M;
+    return 0;
+}
 
 namespace {
 
@@ -568,16 +628,19 @@ float elapsed(cudaEvent_t a, cudaEvent_t b) {
 
 namespace {
 
-// the tables, buffers, streams and events of a run; the generator's state is boost::mt19937(seed), or `state` (625
-// words) when given
-int sim_setup(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p, const uint32_t* state) {
-    sim_free(ctx);
-    SimState* s = new SimState();
-    ctx->sim = s;
+// the tables and buffers of a run on the context's kept state; the generator's state is boost::mt19937(seed), or `state`
+// (625 words) when given.  G > 1: the run is one of G contexts of sim_begin_devices, which also needs the jump scratch.
+int sim_setup(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p, const uint32_t* state, int G) {
+    SimState* s = nullptr;
+    if (int rc = sim_state(ctx, &s)) return rc;
+    sim_stop(ctx);
     const int M = p->M;
     const bool q = p->model_type & 1, paired = p->model_type >= 2;
-    auto fail = [&]() { set_error("sim_begin: cudaMalloc / cudaMemcpy failed"); sim_free(ctx); return RSEM_B200_ERR_CUDA; };
+    const bool own_refs = p->seq != nullptr;
+    RB_ARG(own_refs || (s->ref_block && s->ref_M == M),
+           "sim_begin: params->seq is NULL and no reference with this M was uploaded (rsem_b200_sim_upload_refs)");
     SimTables& t = s->t;
+    t = SimTables{};
     t.type = p->model_type;
     t.M = M;
     t.ori0 = p->ori_prob0;
@@ -587,26 +650,17 @@ int sim_setup(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p, const uint32_t*
     t.mld_lb = p->has_mld ? p->mld.lb : 0;
     t.mld_ub = p->has_mld ? p->mld.ub : 0;
     t.est_rspd = p->est_rspd;
-    const uint64_t total_seq = p->seq_off[M + 1];
-    if (!(t.theta_cdf = dev_copy(p->theta_cdf, (size_t)M + 1, s->owned))) return fail();
-    if (!(t.gld_cdf = dev_copy(p->gld.cdf, (size_t)p->gld.span + 1, s->owned))) return fail();
-    if (p->has_mld && !(t.mld_cdf = dev_copy(p->mld.cdf, (size_t)p->mld.span + 1, s->owned))) return fail();
-    if (p->est_rspd) {
-        if (!(t.rspd_off = dev_copy(p->rspd_off, (size_t)M + 2, s->owned))) return fail();
-        if (!(t.rspd_cdf = dev_copy(p->rspd_cdf, (size_t)p->rspd_off[M + 1], s->owned))) return fail();
-    }
-    if (q) {
-        if (!(t.qd_init = dev_copy(p->qd_init_cdf, kQ, s->owned))) return fail();
-        if (!(t.qd_tran = dev_copy(p->qd_tran_cdf, (size_t)kQ * kQ, s->owned))) return fail();
-    }
-    if (!(t.pro = dev_copy(p->profile_cdf, (size_t)p->pro_rows * 25, s->owned))) return fail();
-    if (!(t.noise = dev_copy(p->noise_cdf, q ? (size_t)kQ * 5 : 5, s->owned))) return fail();
-    if (!(t.seq_off = dev_copy(p->seq_off, (size_t)M + 2, s->owned))) return fail();
-    if (!(t.seq = dev_copy(p->seq, (size_t)total_seq, s->owned))) return fail();
-    if (!(t.tot_len = dev_copy(p->tot_len, (size_t)M + 1, s->owned))) return fail();
-    if (!(t.full_len = dev_copy(p->full_len, (size_t)M + 1, s->owned))) return fail();
     s->exact_body = p->exact_body != 0;
     s->N = p->N;
+    s->done = s->resim = 0;
+    s->entry = 0;
+    s->window = 0;
+    s->slot = 0;
+    s->stats = rsem_b200_sim_stats{};
+    s->G = G;
+    s->gen_pos = s->step_blocks = 0;
+    s->step_nb[0] = s->step_nb[1] = 0;
+    s->jump_ms = 0;
 
     // longest attempt: every draw takes at most 2 words; draws = sid, dir, length, position, 2 mate lengths, and per
     // mate max(len, 1) qualities + len bases
@@ -617,57 +671,113 @@ int sim_setup(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p, const uint32_t*
     W = std::max<uint64_t>(W, s->L);
     RB_ARG(W < 0x7fffffffu - s->L, "window too large");
     s->W = (uint32_t)W;
+    s->K = 0;
     while (((uint64_t)1 << (s->K + 1)) <= W) ++s->K;  // 2^(K+1) > W >= any chain length
     // a successful attempt takes at least 2 words (the sid draw and one more), and a window holds at most N reads
     s->R = (uint32_t)std::min<uint64_t>(W / 2 + 1, std::max<uint64_t>(s->N, 1));
+    s->jump.assign(s->K + 1, nullptr);
+    size_t need = 0, tmp = 0;
+    RB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp, (uint64_t*)nullptr, (uint64_t*)nullptr, (int)s->R + 1, ctx->stream));
+    need = std::max(need, tmp);
+    RB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)s->W, ctx->stream));
+    need = std::max(need, tmp);
+    RB_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, thrust::counting_iterator<uint32_t>(0), (uint8_t*)nullptr,
+                                       (uint32_t*)nullptr, (uint32_t*)nullptr, (int)s->W, ctx->stream));
+    need = std::max(need, tmp);
+    s->scan_tmp_bytes = need;
+
+    // every table and buffer of the run in one arena: the first pass (base nullptr) sizes it, the second points into it
+    const uint64_t total_seq = own_refs ? p->seq_off[M + 1] : 0;
+    struct Upload { void* dst; const void* src; size_t bytes; };
+    std::vector<Upload> up;
+    auto layout = [&](char* base) {
+        size_t off = 0;
+        auto carve = [&](auto*& ptr, size_t n, const void* src = nullptr) {
+            using T = std::remove_cv_t<std::remove_reference_t<decltype(*ptr)>>;
+            off = (off + 255) & ~(size_t)255;
+            T* at = base ? reinterpret_cast<T*>(base + off) : nullptr;
+            ptr = at;
+            if (base && src && n) up.push_back({at, src, n * sizeof(T)});
+            off += std::max<size_t>(n, 1) * sizeof(T);
+        };
+        carve(t.theta_cdf, (size_t)M + 1, p->theta_cdf);
+        carve(t.gld_cdf, (size_t)p->gld.span + 1, p->gld.cdf);
+        if (p->has_mld) carve(t.mld_cdf, (size_t)p->mld.span + 1, p->mld.cdf);
+        if (p->est_rspd) {
+            carve(t.rspd_off, (size_t)M + 2, p->rspd_off);
+            carve(t.rspd_cdf, (size_t)p->rspd_off[M + 1], p->rspd_cdf);
+        }
+        if (q) {
+            carve(t.qd_init, kQ, p->qd_init_cdf);
+            carve(t.qd_tran, (size_t)kQ * kQ, p->qd_tran_cdf);
+        }
+        carve(t.pro, (size_t)p->pro_rows * 25, p->profile_cdf);
+        carve(t.noise, q ? (size_t)kQ * 5 : 5, p->noise_cdf);
+        if (own_refs) {
+            carve(t.seq_off, (size_t)M + 2, p->seq_off);
+            carve(t.seq, (size_t)total_seq, p->seq);
+            carve(t.tot_len, (size_t)M + 1, p->tot_len);
+            carve(t.full_len, (size_t)M + 1, p->full_len);
+        }
+        carve(s->mt, (size_t)kMtN + 1);
+        carve(s->words[0], (size_t)s->W + s->L);
+        carve(s->words[1], (size_t)s->W + s->L);
+        carve(s->len, s->W);
+        for (auto& j : s->jump) carve(j, (size_t)s->W + 1);
+        carve(s->mark, (size_t)s->W + 1);
+        carve(s->chain, s->W);
+        carve(s->n_chain, 1);
+        carve(s->cum, s->W);
+        carve(s->starts, s->R);
+        carve(s->io, 3);
+        carve(s->heads, s->R);
+        carve(s->bytes[0], (size_t)s->R + 1);
+        carve(s->bytes[1], (size_t)s->R + 1);
+        carve(s->counts, (size_t)M + 1);
+        char* scan = nullptr;
+        carve(scan, s->scan_tmp_bytes);
+        s->scan_tmp = scan;
+        if (G > 1) {
+            for (auto& sp : s->step_poly) carve(sp, (size_t)kMtJumpBlocks * kMtBlockWords);
+            carve(s->jump_conv, (size_t)kMtJumpBlocks * kMtN);
+        }
+        return off;
+    };
+    const size_t bytes = layout(nullptr);
+    if (bytes > s->arena_bytes) {  // the only allocation of a run, when it needs more than every run before it
+        cudaFree(s->arena);
+        s->arena = nullptr;
+        s->arena_bytes = 0;
+        RB_CUDA(cudaMalloc(&s->arena, bytes));
+        s->arena_bytes = bytes;
+    }
+    layout(s->arena);
+    if (!own_refs) {
+        t.seq_off = s->ref_seq_off;
+        t.seq = s->ref_seq;
+        t.tot_len = s->ref_tot_len;
+        t.full_len = s->ref_full_len;
+    }
 
     std::vector<uint32_t> mt(kMtN + 1);  // boost::mt19937(seed) (mersenne_twister.hpp seed())
     mt[0] = p->seed;
     for (int i = 1; i < kMtN; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
     mt[kMtN] = kMtN;
     if (state) mt.assign(state, state + kMtN + 1);
-    if (!(s->mt = dev_copy(mt.data(), mt.size(), s->owned))) return fail();
-    SIM_ALLOC(s->words[0], (size_t)s->W + s->L);
-    SIM_ALLOC(s->words[1], (size_t)s->W + s->L);
-    SIM_ALLOC(s->len, s->W);
-    s->jump.resize(s->K + 1);
-    for (auto& j : s->jump) SIM_ALLOC(j, (size_t)s->W + 1);
-    SIM_ALLOC(s->mark, (size_t)s->W + 1);
-    SIM_ALLOC(s->chain, s->W);
-    SIM_ALLOC(s->n_chain, 1);
-    SIM_ALLOC(s->cum, s->W);
-    SIM_ALLOC(s->starts, s->R);
-    SIM_ALLOC(s->io, 3);
-    SIM_ALLOC(s->heads, s->R);
-    SIM_ALLOC(s->bytes[0], (size_t)s->R + 1);
-    SIM_ALLOC(s->bytes[1], (size_t)s->R + 1);
-    SIM_ALLOC(s->counts, (size_t)M + 1);
+    up.push_back({s->mt, mt.data(), mt.size() * sizeof(uint32_t)});
+    for (const Upload& u : up) RB_CUDA(cudaMemcpyAsync(u.dst, u.src, u.bytes, cudaMemcpyHostToDevice, ctx->stream));
     RB_CUDA(cudaMemsetAsync(s->counts, 0, ((size_t)M + 1) * sizeof(double), ctx->stream));
-    size_t need = 0, tmp = 0;
-    RB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp, s->bytes[0], s->bytes[0], (int)s->R + 1, ctx->stream));
-    need = std::max(need, tmp);
-    RB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp, s->cum, s->cum, (int)s->W, ctx->stream));
-    need = std::max(need, tmp);
-    RB_CUDA(cub::DeviceSelect::Flagged(nullptr, tmp, thrust::counting_iterator<uint32_t>(0), s->mark, s->chain,
-                                       s->n_chain, (int)s->W, ctx->stream));
-    need = std::max(need, tmp);
-    s->scan_tmp_bytes = need;
-    RB_CUDA(cudaMalloc(&s->scan_tmp, std::max<size_t>(need, 1)));
-    s->owned.push_back(s->scan_tmp);
-
-    RB_CUDA(cudaStreamCreateWithFlags(&s->gen_stream, cudaStreamNonBlocking));
-    for (auto& e : s->gen_ev) for (cudaEvent_t& x : e) RB_CUDA(cudaEventCreate(&x));
-    for (cudaEvent_t& x : s->used_ev) RB_CUDA(cudaEventCreate(&x));
-    for (cudaEvent_t& x : s->ph_ev) RB_CUDA(cudaEventCreate(&x));
     RB_CUDA(cudaEventRecord(s->used_ev[0], ctx->stream));  // the buffers are free; counts are zeroed first
     RB_CUDA(cudaEventRecord(s->used_ev[1], ctx->stream));
+    RB_CUDA(cudaStreamSynchronize(ctx->stream));  // the tables are on the device before the host's copies go away
+    s->running = true;
     return 0;
 }
 
 }  // namespace
 
 int sim_begin(rsem_b200_ctx* ctx, const rsem_b200_sim_params* p) {
-    if (int rc = sim_setup(ctx, p, nullptr)) return rc;
+    if (int rc = sim_setup(ctx, p, nullptr, 1)) return rc;
     if (int rc = sim_enqueue_gen(ctx->sim, 0)) return rc;
     ctx->launches += 1;
     return 0;
@@ -724,16 +834,15 @@ int sim_emit(rsem_b200_ctx* ctx, SimState* s, int b, uint32_t n, uint64_t rid0, 
         RB_CUDA(cudaMemcpyAsync(&tot[m], s->bytes[m] + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     }
     RB_CUDA(cudaStreamSynchronize(st));
-    const size_t need = std::max(tot[0], tot[1]);
-    if (need > s->text_cap) {
-        RB_CUDA(cudaStreamSynchronize(st));
-        cudaFree(s->text_d[0]);
-        cudaFree(s->text_d[1]);
-        s->text_d[0] = s->text_d[1] = nullptr;
-        s->text_cap = need + need / 4;
-        RB_CUDA(cudaMalloc(&s->text_d[0], s->text_cap));
-        if (paired) RB_CUDA(cudaMalloc(&s->text_d[1], s->text_cap));
-    }
+    // each mate's buffer grows on its own: the context's runs may alternate single-end and paired-end models
+    for (int m = 0; m < nm; ++m)
+        if (tot[m] > s->text_cap[m]) {
+            cudaFree(s->text_d[m]);
+            s->text_d[m] = nullptr;
+            s->text_cap[m] = 0;
+            RB_CUDA(cudaMalloc(&s->text_d[m], tot[m] + tot[m] / 4));
+            s->text_cap[m] = tot[m] + tot[m] / 4;
+        }
     sim_write_kernel<<<gb, kTb, 0, st>>>(s->t, words, s->starts, n, rid0, s->heads, s->bytes[0], s->bytes[1],
                                          s->text_d[0], s->text_d[1], s->counts);
     RB_CUDA(cudaEventRecord(s->ph_ev[2], st));
@@ -759,7 +868,7 @@ int sim_emit(rsem_b200_ctx* ctx, SimState* s, int b, uint32_t n, uint64_t rid0, 
 
 int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_t* n_reads) {
     SimState* s = ctx->sim;
-    RB_ARG(s, "sim_begin must be called first");
+    RB_ARG(s && s->running, "sim_begin must be called first");
     cudaStream_t st = ctx->stream;
     *n_reads = 0;
     bytes[0] = bytes[1] = 0;
@@ -798,11 +907,14 @@ int sim_next(rsem_b200_ctx* ctx, const char* text[2], uint64_t bytes[2], uint64_
 
 int sim_end(rsem_b200_ctx* ctx, double* counts, uint64_t* resim, rsem_b200_sim_stats* stats) {
     SimState* s = ctx->sim;
-    RB_ARG(s, "sim_begin must be called first");
-    if (counts) RB_CUDA(cudaMemcpy(counts, s->counts, ((size_t)s->t.M + 1) * sizeof(double), cudaMemcpyDeviceToHost));
+    RB_ARG(s && s->running, "sim_begin must be called first");
+    if (counts) {
+        RB_CUDA(cudaMemcpyAsync(counts, s->counts, ((size_t)s->t.M + 1) * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        RB_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
     if (resim) *resim = s->resim;
     if (stats) { s->stats.windows = s->window; *stats = s->stats; }
-    sim_free(ctx);
+    sim_stop(ctx);
     return 0;
 }
 
@@ -850,10 +962,10 @@ int sim_enqueue_prep(rsem_b200_ctx* ctx, SimState* s, uint64_t lw) {
     return 0;
 }
 
-void free_all(const std::vector<rsem_b200_ctx*>& ctxs) {
+void stop_all(const std::vector<rsem_b200_ctx*>& ctxs) {
     for (rsem_b200_ctx* c : ctxs) {
         cudaSetDevice(c->device);
-        sim_free(c);
+        sim_stop(c);
     }
 }
 
@@ -875,9 +987,9 @@ int sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_par
     int step_nb[2] = {0, 0};
     for (int g = 0; g < n; ++g) {
         rsem_b200_ctx* ctx = ctxs[g];
-        auto fail = [&](int rc) { free_all(m->ctx); return rc; };
+        auto fail = [&](int rc) { stop_all(m->ctx); return rc; };
         if (cudaSetDevice(ctx->device) != cudaSuccess) return fail(cuda_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__));
-        if (int rc = sim_setup(ctx, p, nullptr)) return fail(rc);
+        if (int rc = sim_setup(ctx, p, nullptr, n)) return fail(rc);
         SimState* s = ctx->sim;
         if (g == 0) {
             const uint64_t J = (uint64_t)(n - 1) * s->W - s->L;
@@ -896,23 +1008,21 @@ int sim_begin_devices(rsem_b200_ctx* const* ctxs, int n, const rsem_b200_sim_par
         s->G = n;
         s->gen_pos = (uint64_t)g * s->W;
         s->step_blocks = step_blocks;
-        if (g > 0) {
-            if (int rc = rsem_b200_mt19937_jump(seeded.data(), s->gen_pos, state.data())) return fail(rc);
-            if (cudaMemcpy(s->mt, state.data(), state.size() * sizeof(uint32_t), cudaMemcpyHostToDevice) != cudaSuccess)
-                return fail(cuda_fail(cudaGetLastError(), "cudaMemcpy", __FILE__, __LINE__));
-        }
-        for (int v = 0; v < 2; ++v) {
-            s->step_nb[v] = step_nb[v];
-            if (step_h[v].empty()) continue;
-            if (!(s->step_poly[v] = dev_copy(step_h[v].data(), step_h[v].size(), s->owned))) {
-                set_error("sim_begin_devices: cudaMalloc / cudaMemcpy failed");
-                return fail(RSEM_B200_ERR_CUDA);
-            }
-        }
         auto setup = [&]() -> int {
-            SIM_ALLOC(s->jump_conv, (size_t)kMtJumpBlocks * kMtN);
-            for (cudaEvent_t& x : s->jump_ev) RB_CUDA(cudaEventCreate(&x));
-            for (auto& e : s->prep_ev) for (cudaEvent_t& x : e) RB_CUDA(cudaEventCreate(&x));
+            if (g > 0) {
+                if (int rc = rsem_b200_mt19937_jump(seeded.data(), s->gen_pos, state.data())) return rc;
+                RB_CUDA(cudaMemcpyAsync(s->mt, state.data(), state.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+            }
+            for (int v = 0; v < 2; ++v) {
+                s->step_nb[v] = step_nb[v];
+                if (!step_h[v].empty())
+                    RB_CUDA(cudaMemcpyAsync(s->step_poly[v], step_h[v].data(), step_h[v].size() * sizeof(uint32_t),
+                                            cudaMemcpyHostToDevice, ctx->stream));
+            }
+            // the generator stream waits for these copies (the buffers' events were recorded before them)
+            RB_CUDA(cudaEventRecord(s->used_ev[0], ctx->stream));
+            RB_CUDA(cudaEventRecord(s->used_ev[1], ctx->stream));
+            RB_CUDA(cudaStreamSynchronize(ctx->stream));
             if (int rc = sim_enqueue_gen_jump(ctx, s, 0)) return rc;
             return sim_enqueue_prep(ctx, s, 0);
         };
@@ -931,7 +1041,7 @@ int sim_next_devices(rsem_b200_sim_multi* m, const char* text[2], uint64_t bytes
         rsem_b200_ctx* ctx = m->ctx[m->window % G];
         RB_CUDA(cudaSetDevice(ctx->device));
         SimState* s = ctx->sim;
-        RB_ARG(s, "sim_begin_devices must be called first");
+        RB_ARG(s && s->running, "sim_begin_devices must be called first");
         cudaStream_t st = ctx->stream;
         const uint64_t lw = s->window;
         const int b = (int)(lw & 1);
@@ -975,8 +1085,8 @@ int sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rse
         rsem_b200_ctx* ctx = m->ctx[g];
         RB_CUDA(cudaSetDevice(ctx->device));
         SimState* s = ctx->sim;
-        if (!s) {
-            free_all(m->ctx);
+        if (!s || !s->running) {
+            stop_all(m->ctx);
             RB_ARG(false, "sim_begin_devices must be called first");
         }
         if (counts && c.empty()) c.assign((size_t)s->t.M + 1, 0.0);
@@ -985,7 +1095,7 @@ int sim_end_devices(rsem_b200_sim_multi* m, double* counts, uint64_t* resim, rse
         uint64_t r = 0;
         rsem_b200_sim_stats st{};
         if (int rc = sim_end(ctx, counts ? cg.data() : nullptr, &r, &st)) {
-            free_all(m->ctx);
+            stop_all(m->ctx);
             return rc;
         }
         for (size_t i = 0; i < c.size(); ++i) c[i] += cg[i];  // integers: any order gives the same sums

@@ -177,8 +177,9 @@ struct HostModel {
     void write(const std::string& path) const;   // Model::write
     // Model::read for rsem-run-gibbs: only gld and mw are needed afterwards, but the whole file is parsed
     static void read_for_gibbs(const std::string& path, int M, int& model_type, LenDistH& gld, std::vector<double>& mw);
-    // the whole .model file, every model type (rsem-simulate-reads); mw stays empty when the file has none for M
-    void read(const std::string& path, int M);
+    // the whole .model file, every model type (rsem-simulate-reads); mw stays empty when the file has none for M.
+    // file_M (optional): the transcript count the file's mw block is written for, 0 when it has none
+    void read(const std::string& path, int M, int* file_M = nullptr);
 };
 
 // ---- O(M) result math (WriteResults.h:24-104) ------------------------------------------------------
@@ -290,6 +291,52 @@ void write_results_gibbs(const std::string& ref_name, const std::string& imd_nam
 void write_results_simulation(const std::string& ref_name, const std::string& out_name,
                               const std::vector<TranscriptInfo>& tr, const std::vector<double>& eel,
                               const std::vector<double>& counts);  // WriteResults.h:481-635
+
+// ---- sim_sample.cpp: the per-sample stages of rsem-simulate-reads, which rsem-simulate-reads-batch runs for each line -----
+struct SimReference {   // refName.seq with the sequences, refName.ti and the allele groups (WriteResults.h:106-123)
+    std::string name;
+    RefData refs;
+    std::vector<TranscriptInfo> transcripts;
+    std::vector<int> gt, ta;
+    bool alleleS = false;
+    int offsite = 5;     // column of the TPM in the results file (simulation.cpp:94-100)
+};
+void load_sim_reference(const std::string& refName, SimReference& ref);
+// rsem-simulate-reads's arguments after reference_name (simulation.cpp:160-182)
+struct SimArgs {
+    std::string modelF, resultsF, outName;
+    double theta0 = 0;
+    long long N = 0;
+    bool hasSeed = false, quiet = false;
+    uint32_t seed = 0;
+};
+// estimated_model_file estimated_isoform_results theta0 N output_name [--seed seed] [-q] (f.size() >= 5): atof theta0,
+// atoi N, istringstream for the seed; returns "" or why the seed cannot be taken
+std::string parse_sim_args(const std::vector<std::string>& f, SimArgs& a);
+// the model type on the first line of a .model file: -1 when the file cannot be opened, -2 when it is not 0..3
+int sim_model_type(const std::string& modelF);
+// the read file(s) a run writes (genOutReadStreams, simulation.cpp:60-84)
+std::vector<std::string> sim_read_files(const std::string& outName, int model_type);
+// what rsem-simulate-reads derives from the model and the results file before it draws (simulation.cpp:86-120)
+struct SimSample {
+    HostModel model;
+    std::vector<double> eel, theta, theta_cdf, qd_init, qd_tran, pro, noise, rspd_cdf;
+    std::vector<uint64_t> rspd_off;
+    int pro_rows = 0;
+    bool exact_body = false;
+};
+// the model, the expected effective lengths, theta and the cumulative tables; false when the results file gives every
+// transcript TPM * effective length 0 (simulation.cpp:113)
+bool load_sim_sample(const SimReference& ref, const SimArgs& a, SimSample& s);
+// the run's parameters; with_seq false leaves the reference out (the context's rsem_b200_sim_upload_refs copy is used).
+// RSEM_B200_SIM_WINDOW sets the window.  The pointers are into ref and s.
+rsem_b200_sim_params sim_params(const SimReference& ref, const SimSample& s, uint32_t seed, long long N, bool with_seq);
+// The chunk loop of a run: next() is rsem_b200_sim_next or _next_devices; the text of one chunk is written to the
+// read files on a second thread while the device produces the next one.  `gen` (may be null) gets the GEN lines
+// (simulation.cpp:125).  Returns the reads written; t_next adds the time in next(), t_write the time spent waiting for
+// the writes.
+using SimNext = std::function<void(const char* text[2], uint64_t bytes[2], uint64_t* n)>;
+uint64_t write_sim_reads(const SimNext& next, FILE* const* os, int n_os, const Say* gen, double& t_next, double& t_write);
 
 // ---- alignment files for -b: SAM / BAM in, BAM out (bam.cpp; BamWriter.h, sam_utils.h, SamHeader.cpp) -----------------
 struct BamRecord {

@@ -548,7 +548,7 @@ void HostModel::read_for_gibbs(const std::string& path, int M, int& model_type, 
 }
 
 // Model::read (SingleModel.h:356-381, SingleQModel.h:383-411, PairedEndModel.h:296-317, PairedEndQModel.h:316-343)
-void HostModel::read(const std::string& path, int M) {
+void HostModel::read(const std::string& path, int M, int* file_M) {
     FILE* fi = fopen(path.c_str(), "r");
     if (!fi) die("Cannot open " + path + "! It may not exist.");
     auto need = [&](bool ok) { if (!ok) die("Cannot parse " + path + "!"); };
@@ -595,7 +595,9 @@ void HostModel::read(const std::string& path, int M) {
     }
     for (double& d : noise_p) need(fscanf(fi, "%lf", &d) == 1);
     mw.clear();
-    if (fscanf(fi, "%d", &v) == 1 && v == M) {
+    const bool has_M = fscanf(fi, "%d", &v) == 1;
+    if (file_M) *file_M = has_M ? v : 0;
+    if (has_M && v == M) {
         mw.resize((size_t)M + 1);
         for (int i = 0; i <= M; ++i) need(fscanf(fi, "%lf", &mw[i]) == 1);
     }
