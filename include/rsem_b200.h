@@ -435,13 +435,16 @@ typedef struct rsem_b200_ci_stats {
     int32_t resident;     /* 1: the sample matrix was kept on the device                                        */
     int32_t reserved;
 } rsem_b200_ci_stats;
-/* allocates the sample matrix (Buffer.h:16-31 sizes a host buffer instead) */
+/* sets up a run and its sample matrix (Buffer.h:16-31 sizes a host buffer instead).  The context keeps K8's buffers
+ * from one run to the next and grows them only when a run needs more, so a run whose shape it has already held makes no
+ * allocation; when the kept buffers would then exceed both the budget and what this run needs, the larger ones are
+ * released first.  With device_budget = 0 the memory the context keeps for K8 counts as free.  ctx_destroy frees them. */
 int rsem_b200_ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* params);
 /* count samples from index first: rows = count x M TPMs (tpm + 1 of calcCI.cpp:146), l_bars = count values.  Thread
  * safe; the buffers may be reused when it returns (Buffer::write, Buffer.h:41-49)                                 */
 int rsem_b200_ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars, int64_t first, int64_t count);
 /* intervals as (lb, ub, cqv) of TPM then of FPKM, 6 floats per item: transcripts (M), genes (n_genes), isoforms
- * (n_isoforms; may be NULL when 0) (calcCI.cpp:313-385, 446-496 prints them); frees the state                     */
+ * (n_isoforms; may be NULL when 0) (calcCI.cpp:313-385, 446-496 prints them); ends the run and keeps its buffers  */
 int rsem_b200_ci_end(rsem_b200_ctx* ctx, float* transcripts, float* genes, float* isoforms, rsem_b200_ci_stats* stats);
 
 /* ---- rsem-for-ebseq-calculate-clustering-info (K9, kmer_kernels.cu) ----------------------------------------------------

@@ -4,7 +4,7 @@
   bin/rsem-run-em, bin/rsem-run-gibbs, bin/rsem-parse-alignments, bin/rsem-simulate-reads,
   bin/rsem-calculate-credibility-intervals, bin/rsem-for-ebseq-calculate-clustering-info, bin/rsem-tbam2gbam,
   bin/rsem-bam2wig, bin/rsem-bam2readdepth, bin/rsem-run-em-batch, bin/rsem-run-gibbs-batch,
-  bin/rsem-simulate-reads-batch
+  bin/rsem-simulate-reads-batch, bin/rsem-calculate-credibility-intervals-batch
                               C++ drop-in executables (link the .so)
   tools/gen_dataset           synthetic intermediate-file generator (tooling)
   oracle/librsem_oracle.so    CPU restatement (test infrastructure)
@@ -54,7 +54,9 @@ def build_host(force: bool = False):
     mains = [s for s in common if os.path.basename(s).startswith("main_")]
     # the simulator's per-sample stages call the tables of ffm/sim_tables.cpp, so only the two simulators link them
     sim_only = [os.path.join(HOST, "sim_sample.cpp")]
-    shared = [s for s in common if s not in mains and s not in sim_only]
+    # likewise the credibility-interval stages call the sampler of ffm/ci_sample.cpp
+    ci_only = [os.path.join(HOST, "ci_stages.cpp")]
+    shared = [s for s in common if s not in mains and s not in sim_only and s not in ci_only]
     # the simulator's tables and the credibility-interval sampler are built in files compiled with the reference's flags
     # for simulation.cpp and calcCI.cpp (-O3 -ffast-math, reference Makefile:39,72-73), so that they carry the same bits;
     # the link step adds no -ffast-math (no crtfastmath.o, which would set flush-to-zero for the whole process)
@@ -75,13 +77,17 @@ def build_host(force: bool = False):
                 "main_tbam2gbam.cpp": "rsem-tbam2gbam", "main_bam2wig.cpp": "rsem-bam2wig",
                 "main_bam2readdepth.cpp": "rsem-bam2readdepth", "main_em_batch.cpp": "rsem-run-em-batch",
                 "main_gibbs_batch.cpp": "rsem-run-gibbs-batch",
-                "main_simulate_batch.cpp": "rsem-simulate-reads-batch"}[os.path.basename(m)]
+                "main_simulate_batch.cpp": "rsem-simulate-reads-batch",
+                "main_ci_batch.cpp": "rsem-calculate-credibility-intervals-batch"}[os.path.basename(m)]
         out = os.path.join(ROOT, "bin", name)
         ffm_use = {"rsem-simulate-reads": "sim_tables.o", "rsem-simulate-reads-batch": "sim_tables.o",
-                   "rsem-calculate-credibility-intervals": "ci_sample.o"}
+                   "rsem-calculate-credibility-intervals": "ci_sample.o",
+                   "rsem-calculate-credibility-intervals-batch": "ci_sample.o"}
         extra = [o for o in ffm_objs if os.path.basename(o) == ffm_use.get(name)]
         if name.startswith("rsem-simulate-reads"):
             extra += sim_only
+        if name.startswith("rsem-calculate-credibility-intervals"):
+            extra += ci_only
         if force or _newer(out, deps + [os.path.join(ROOT, "rsem_b200", "librsem_b200.so")]):
             _run(["g++", "-O2", "-std=c++17", "-Wall", "-pthread", "-I", os.path.join(ROOT, "include"), "-o", out, m, *shared, *extra,
                   "-L", os.path.join(ROOT, "rsem_b200"), "-lrsem_b200", "-Wl,-rpath,$ORIGIN/../rsem_b200",

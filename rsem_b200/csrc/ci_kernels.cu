@@ -14,6 +14,9 @@
 //               hinges and the coefficient of quartile variation, in the reference's float / double mix
 // Results go back as (lb, ub, cqv) per row.  Every float operation uses explicit round-to-nearest intrinsics, so no
 // contraction into an FMA changes a bit.
+// The context keeps every buffer of a run (the matrix, l_bars, pinned stages, the block buffers and CUB's storage) after
+// ci_end and grows each only when a later run needs more: cudaFree / cudaFreeHost synchronise the whole device, under
+// the other lanes of rsem-calculate-credibility-intervals-batch.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -158,33 +161,79 @@ int blocks_for(const rsem_b200_ctx* ctx, int64_t total) {
 
 }  // namespace
 
+// A buffer kept on the context from one run to the next: device memory, or pinned host memory for a sample matrix that
+// stays in host memory.  It is reallocated only when a run needs more than it holds.
+struct Kept {
+    void* p = nullptr;
+    size_t cap = 0;
+};
+
+// K8's device buffers, kept on the context after ci_end
+enum { kS, kLbar, kX, kY, kCol, kOff, kGb, kGe, kRes, kIsoRes, kIso0, kIso1, kIso2, kIso3, kTmp, kDevBuffers };
+
 struct CiState {
+    // the run between ci_begin and ci_end
+    bool active = false;
     int M = 0, m = 0, threshold = 0;
     int64_t n = 0;
     std::vector<int> gene_start, iso_start, part_gene;  // 1-based transcript ids as GroupInfo holds them
     bool resident = true;
-    float* S = nullptr;       // n x M, device (resident) or pinned host
+    float* S = nullptr;       // n x M: dev[kS] (resident) or host_S
     std::vector<float> lbar_h;
-    float* lbar = nullptr;    // n, device
-    char* stage[2] = {nullptr, nullptr};
-    cudaEvent_t stage_ev[2] = {nullptr, nullptr};
+    float* lbar = nullptr;    // n, device: dev[kLbar]
     int next_stage = 0;
     uint64_t budget = 0;
+    int64_t rows_cap = 0;     // rows of one block of the walk
     std::mutex mu;
     rsem_b200_ci_stats stats{};
+    // kept from run to run; ctx_destroy frees them
+    Kept dev[kDevBuffers];
+    Kept host_S;
+    char* stage[2] = {nullptr, nullptr};
+    cudaEvent_t stage_ev[2] = {nullptr, nullptr};
+    cudaEvent_t ev[6] = {};
 };
+
+namespace {
+
+uint64_t held_device_bytes(const CiState* s) {
+    uint64_t b = 0;
+    for (const Kept& k : s->dev) b += k.cap;
+    return b;
+}
+
+void release(Kept& k, bool host) {
+    if (k.p) {
+        if (host) cudaFreeHost(k.p); else cudaFree(k.p);
+    }
+    k = Kept{};
+}
+
+// k holds at least `bytes` (0: not needed by this run; whatever k holds is kept)
+cudaError_t ensure(Kept& k, size_t bytes, bool host = false) {
+    if (bytes == 0 || k.cap >= bytes) return cudaSuccess;
+    release(k, host);
+    cudaError_t e = host ? cudaHostAlloc(&k.p, bytes, cudaHostAllocDefault) : cudaMalloc(&k.p, bytes);
+    if (e == cudaSuccess) k.cap = bytes;
+    else k.p = nullptr;
+    return e;
+}
+
+}  // namespace
 
 void ci_free(rsem_b200_ctx* ctx) {
     CiState* s = ctx->ci;
     if (!s) return;
     cudaStreamSynchronize(ctx->copy_stream);
     cudaStreamSynchronize(ctx->stream);
-    if (s->resident) cudaFree(s->S); else cudaFreeHost(s->S);
-    cudaFree(s->lbar);
+    for (Kept& k : s->dev) release(k, false);
+    release(s->host_S, true);
     for (int b = 0; b < 2; ++b) {
         if (s->stage[b]) cudaFreeHost(s->stage[b]);
         if (s->stage_ev[b]) cudaEventDestroy(s->stage_ev[b]);
     }
+    for (auto& e : s->ev)
+        if (e) cudaEventDestroy(e);
     delete s;
     ctx->ci = nullptr;
 }
@@ -200,24 +249,57 @@ int64_t gene_rows(const CiState* s, int g) {
 // bytes a block of `rows` rows needs besides S: the rows, CUB's alternate buffer, column staging for a host-resident S
 int64_t block_bytes_per_row(const CiState* s) { return s->n * 4 * (s->resident ? 2 : 3); }
 
+// the bytes of each kept device buffer this run uses (0: not used), with the blocks of rows_cap rows of ci_end
+void device_needs(const CiState* s, size_t need[kDevBuffers]) {
+    const int64_t n = s->n, rows_cap = s->rows_cap;
+    const size_t row_b = (size_t)n * 4;
+    auto at_least = [](size_t b) { return std::max<size_t>(b, 16); };
+    for (int i = 0; i < kDevBuffers; ++i) need[i] = 0;
+    need[kS] = s->resident ? (size_t)n * s->M * 4 : 0;
+    need[kLbar] = row_b;
+    int64_t max_rows = 0;
+    for (int g = 0; g < s->m; ++g) max_rows = std::max(max_rows, gene_rows(s, g));
+    if (rows_cap < max_rows) return;  // ci_end refuses the run before it needs a block
+    need[kX] = need[kY] = at_least(rows_cap * row_b);
+    if (!s->resident) need[kCol] = at_least(rows_cap * row_b);
+    need[kOff] = at_least((rows_cap + 1) * sizeof(int64_t));
+    need[kGb] = need[kGe] = at_least(rows_cap * sizeof(int));
+    need[kRes] = at_least(rows_cap * 3 * sizeof(float));
+    need[kIsoRes] = at_least(6 * sizeof(float));
+    if (!s->iso_start.empty())
+        for (int i = kIso0; i <= kIso3; ++i) need[i] = at_least(row_b);
+    size_t seg = 0, one = 0;
+    cub::DoubleBuffer<float> keys(nullptr, nullptr);
+    cub::DeviceSegmentedSort::SortKeys(nullptr, seg, keys, (int)(rows_cap * n), (int)rows_cap, (int64_t*)nullptr,
+                                       (int64_t*)nullptr + 1);
+    cub::DeviceRadixSort::SortKeys(nullptr, one, keys, (int)n, 0, 32);
+    need[kTmp] = at_least(std::max(seg, one));
+}
+
 }  // namespace
 
 int ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* p) {
-    ci_free(ctx);
-    CiState* s = new CiState();
-    ctx->ci = s;
+    if (!ctx->ci) ctx->ci = new CiState();
+    CiState* s = ctx->ci;
+    RB_CUDA(cudaStreamSynchronize(ctx->copy_stream));  // a run begun again before its ci_end
+    RB_CUDA(cudaStreamSynchronize(ctx->stream));
+    s->active = false;
     s->M = p->M;
     s->m = p->n_genes;
     s->n = p->n_samples;
     s->threshold = p->threshold;
     s->gene_start.assign(p->gene_start, p->gene_start + p->n_genes + 1);
+    s->iso_start.clear();
     if (p->n_isoforms > 0) s->iso_start.assign(p->isoform_start, p->isoform_start + p->n_isoforms + 1);
     s->part_gene.assign(p->part_gene_start, p->part_gene_start + p->n_parts + 1);
     s->lbar_h.assign(s->n, 0.0f);
+    s->next_stage = 0;
+    s->stats = rsem_b200_ci_stats{};
     size_t free_b = 0, total_b = 0;
     RB_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const uint64_t reserve = 512ull << 20;
-    s->budget = p->device_budget ? p->device_budget : (free_b > reserve ? free_b - reserve : 0);
+    const uint64_t avail = free_b + held_device_bytes(s);  // what this context keeps for K8 is this run's to use
+    s->budget = p->device_budget ? p->device_budget : (avail > reserve ? avail - reserve : 0);
     int64_t max_rows = 0;
     for (int g = 0; g < s->m; ++g) max_rows = std::max(max_rows, gene_rows(s, g));
     const int64_t s_bytes = s->n * (int64_t)s->M * 4;
@@ -225,26 +307,53 @@ int ci_begin(rsem_b200_ctx* ctx, const rsem_b200_ci_params* p) {
     s->resident = (int64_t)s->budget >= s_bytes + fixed + max_rows * s->n * 8;
     if (!s->resident && (int64_t)s->budget < fixed + max_rows * s->n * 12) {
         set_error("ci_begin: the device budget cannot hold the rows of the largest gene");
-        ci_free(ctx);
         return RSEM_B200_ERR_ARG;
     }
+    // block capacity from what the budget leaves next to S
+    s->rows_cap = ((int64_t)s->budget - (s->resident ? s_bytes : 0) - fixed) / block_bytes_per_row(s);
+    s->rows_cap = std::min<int64_t>(s->rows_cap, (int64_t)INT32_MAX / s->n);
+    int64_t all_rows = 0;
+    for (int g = 0; g < s->m; ++g) all_rows += gene_rows(s, g);
+    s->rows_cap = std::min(s->rows_cap, all_rows);
+
+    // The kept buffers this run leaves in place or grows.  When what they would then hold exceeds both the budget and
+    // what this run needs, the ones larger than this run needs are released first (largest first) until it does not.
+    size_t need[kDevBuffers];
+    device_needs(s, need);
+    uint64_t after = 0, needed = 0;
+    for (int i = 0; i < kDevBuffers; ++i) {
+        after += std::max(s->dev[i].cap, need[i]);
+        needed += need[i];
+    }
+    const uint64_t limit = std::max<uint64_t>(s->budget, needed);
+    while (after > limit) {
+        int big = -1;
+        for (int i = 0; i < kDevBuffers; ++i)
+            if (s->dev[i].cap > need[i] && (big < 0 || s->dev[i].cap - need[i] > s->dev[big].cap - need[big])) big = i;
+        after -= s->dev[big].cap - need[big];
+        release(s->dev[big], false);
+    }
     if (s->resident) {
-        RB_CUDA(cudaMalloc(&s->S, (size_t)s_bytes));
+        RB_CUDA(ensure(s->dev[kS], need[kS]));
+        s->S = (float*)s->dev[kS].p;
         for (int b = 0; b < 2; ++b) {
-            RB_CUDA(cudaHostAlloc(&s->stage[b], kStageBytes, cudaHostAllocDefault));
-            RB_CUDA(cudaEventCreateWithFlags(&s->stage_ev[b], cudaEventDisableTiming));
+            if (!s->stage[b]) RB_CUDA(cudaHostAlloc(&s->stage[b], kStageBytes, cudaHostAllocDefault));
+            if (!s->stage_ev[b]) RB_CUDA(cudaEventCreateWithFlags(&s->stage_ev[b], cudaEventDisableTiming));
         }
     } else {
-        RB_CUDA(cudaHostAlloc(&s->S, (size_t)s_bytes, cudaHostAllocDefault));
+        RB_CUDA(ensure(s->host_S, (size_t)s_bytes, true));
+        s->S = (float*)s->host_S.p;
     }
-    RB_CUDA(cudaMalloc(&s->lbar, (size_t)s->n * 4));
+    RB_CUDA(ensure(s->dev[kLbar], need[kLbar]));
+    s->lbar = (float*)s->dev[kLbar].p;
     s->stats.resident = s->resident;
+    s->active = true;
     return 0;
 }
 
 int ci_push(rsem_b200_ctx* ctx, const float* rows, const float* l_bars, int64_t first, int64_t count) {
     CiState* s = ctx->ci;
-    RB_ARG(s, "ci_begin must be called first");
+    RB_ARG(s && s->active, "ci_begin must be called first");
     RB_ARG(first >= 0 && count >= 0 && first + count <= s->n, "samples out of range");
     std::lock_guard<std::mutex> lock(s->mu);
     memcpy(&s->lbar_h[first], l_bars, (size_t)count * 4);
@@ -314,7 +423,7 @@ int ci_finish_isoform(rsem_b200_ctx* ctx, Work& wk, float* out_h) {
 
 int ci_end(rsem_b200_ctx* ctx, float* tr_out, float* gene_out, float* iso_out, rsem_b200_ci_stats* stats) {
     CiState* s = ctx->ci;
-    RB_ARG(s, "ci_begin must be called first");
+    RB_ARG(s && s->active, "ci_begin must be called first");
     RB_ARG(s->iso_start.empty() || iso_out, "isoforms is NULL for an allele-specific reference");
     cudaStream_t st = ctx->stream;
     const int64_t n = s->n;
@@ -322,34 +431,12 @@ int ci_end(rsem_b200_ctx* ctx, float* tr_out, float* gene_out, float* iso_out, r
     RB_CUDA(cudaStreamSynchronize(ctx->copy_stream));
     RB_CUDA(cudaMemcpyAsync(s->lbar, s->lbar_h.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
 
-    // block capacity from what the budget leaves next to S
-    const int64_t s_bytes = s->resident ? n * (int64_t)M * 4 : 0;
-    const int64_t fixed = n * 4 * (1 + 4) + (1 << 20);
-    int64_t rows_cap = ((int64_t)s->budget - s_bytes - fixed) / block_bytes_per_row(s);
-    rows_cap = std::min<int64_t>(rows_cap, (int64_t)INT32_MAX / n);
-    int64_t max_rows = 0, all_rows = 0;
-    for (int g = 0; g < s->m; ++g) {
-        max_rows = std::max(max_rows, gene_rows(s, g));
-        all_rows += gene_rows(s, g);
-    }
-    rows_cap = std::min(rows_cap, all_rows);
+    const int64_t rows_cap = s->rows_cap;
+    int64_t max_rows = 0;
+    for (int g = 0; g < s->m; ++g) max_rows = std::max(max_rows, gene_rows(s, g));
     RB_ARG(rows_cap >= max_rows, "ci_end: the device budget cannot hold the rows of the largest gene");
 
-    Work wk;
-    std::vector<void*> owned;
-    auto alloc = [&](auto** p, size_t bytes) {
-        cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(bytes, 16));
-        if (e == cudaSuccess) owned.push_back((void*)*p);
-        return e;
-    };
-    auto release = [&]() { for (void* q : owned) cudaFree(q); };
-    cudaEvent_t ev[6];
-    for (auto& e : ev) cudaEventCreate(&e);
-    auto cleanup = [&]() {
-        cudaStreamSynchronize(st);
-        release();
-        for (auto& e : ev) cudaEventDestroy(e);
-    };
+    auto cleanup = [&]() { cudaStreamSynchronize(st); };
 #define CI_CUDA(call)                                                                 \
     do {                                                                              \
         cudaError_t _e = (call);                                                      \
@@ -359,27 +446,27 @@ int ci_end(rsem_b200_ctx* ctx, float* tr_out, float* gene_out, float* iso_out, r
         }                                                                             \
     } while (0)
     const size_t row_b = (size_t)n * 4;
-    CI_CUDA(alloc(&wk.X, rows_cap * row_b));
-    CI_CUDA(alloc(&wk.Y, rows_cap * row_b));
-    if (!s->resident) CI_CUDA(alloc(&wk.col, rows_cap * row_b));
-    CI_CUDA(alloc(&wk.off, (rows_cap + 1) * sizeof(int64_t)));
-    CI_CUDA(alloc(&wk.gb, rows_cap * sizeof(int)));
-    CI_CUDA(alloc(&wk.ge, rows_cap * sizeof(int)));
-    CI_CUDA(alloc(&wk.res, rows_cap * 3 * sizeof(float)));
-    CI_CUDA(alloc(&wk.iso_res, 6 * sizeof(float)));
+    size_t need[kDevBuffers];
+    device_needs(s, need);
+    for (int i = kX; i < kDevBuffers; ++i) CI_CUDA(ensure(s->dev[i], need[i]));
+    for (auto& e : s->ev)
+        if (!e) CI_CUDA(cudaEventCreate(&e));
+    cudaEvent_t* ev = s->ev;
+    Work wk;
+    wk.X = (float*)s->dev[kX].p;
+    wk.Y = (float*)s->dev[kY].p;
+    wk.col = (float*)s->dev[kCol].p;
+    wk.off = (int64_t*)s->dev[kOff].p;
+    wk.gb = (int*)s->dev[kGb].p;
+    wk.ge = (int*)s->dev[kGe].p;
+    wk.res = (float*)s->dev[kRes].p;
+    wk.iso_res = (float*)s->dev[kIsoRes].p;
+    wk.tmp = s->dev[kTmp].p;
+    wk.tmp_bytes = need[kTmp];
     const bool alleles = !s->iso_start.empty();
     if (alleles)
-        for (auto& a : wk.iso)
-            for (auto& b : a) CI_CUDA(alloc(&b, row_b));
-    {
-        size_t seg = 0, one = 0;
-        cub::DoubleBuffer<float> keys(wk.X, wk.Y);
-        CI_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, seg, keys, (int)(rows_cap * n), (int)rows_cap, wk.off,
-                                                   wk.off + 1, st));
-        CI_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, one, keys, (int)n, 0, 32, st));
-        wk.tmp_bytes = std::max(seg, one);
-        CI_CUDA(alloc(&wk.tmp, wk.tmp_bytes));
-    }
+        for (int a = 0; a < 2; ++a)
+            for (int b = 0; b < 2; ++b) wk.iso[a][b] = (float*)s->dev[kIso0 + 2 * a + b].p;
 
     // isoform chain state (calcCI.cpp:307-373): allele id -> isoform id, and every isoform result in the order the
     // reference assigns it (an isoform may be assigned twice when it straddles two Phase II thread ranges)
@@ -523,7 +610,7 @@ int ci_end(rsem_b200_ctx* ctx, float* tr_out, float* gene_out, float* iso_out, r
 #undef CI_CUDA
     cleanup();
     if (stats) *stats = s->stats;
-    ci_free(ctx);
+    s->active = false;
     return 0;
 }
 

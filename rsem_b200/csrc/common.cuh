@@ -280,7 +280,7 @@ struct rsem_b200_ctx {
 
     rsem_b200::DevGibbs gibbs;
     rsem_b200::SimState* sim = nullptr;  // rsem-simulate-reads: the run, its kept buffers and the uploaded reference
-    rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals between ci_begin and ci_end
+    rsem_b200::CiState* ci = nullptr;    // rsem-calculate-credibility-intervals: the run and its kept buffers
     rsem_b200::GbamState* gbam = nullptr;  // rsem-tbam2gbam: transcript tables and batch scratch
     rsem_b200::WigState* wig = nullptr;    // rsem-bam2wig / rsem-bam2readdepth: the resident run and batch scratch
 

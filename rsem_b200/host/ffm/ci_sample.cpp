@@ -10,8 +10,8 @@
 // this compiler decides.
 #include <cmath>
 #include <cstdint>
-#include <cstdio>
 #include <random>
+#include <string>
 #include <vector>
 
 #include "../host.hpp"
@@ -61,9 +61,10 @@ double gamma_draw(std::mt19937& eng, double alpha, double p) {
 }  // namespace
 
 // cvs: n_cv count vectors of M + 1 entries (-1 = omitted).  emit(sample, tpm[1..M], l_bar) for the nSpC samples of each
-// vector in order; `sample` counts from 0 within this file.  Progress lines as calcCI.cpp:154 when `verbose`.
+// vector in order; `sample` counts from 0 within this file.  Progress lines as calcCI.cpp:154 go to `progress` (none
+// when it is null).
 void ci_sample_vectors(const int32_t* cvs, int n_cv, int M, int nSpC, double pseudoC, uint32_t seed, const double* eel,
-                       const double* mw, int thread_no, bool verbose,
+                       const double* mw, int thread_no, const Say* progress,
                        const std::function<void(int64_t, const float*, float)>& emit) {
     std::mt19937 eng(seed);
     std::vector<double> theta(M + 1), alpha(M + 1), p(M + 1);
@@ -106,7 +107,8 @@ void ci_sample_vectors(const int32_t* cvs, int n_cv, int M, int nSpC, double pse
             }
             emit(sample++, tpm.data() + 1, l_bar);
         }
-        if (verbose && (c + 1) % 100 == 0) printf("Thread %d, %d count vectors are processed!\n", thread_no, c + 1);
+        if (progress && (c + 1) % 100 == 0)
+            (*progress)("Thread " + std::to_string(thread_no) + ", " + std::to_string(c + 1) + " count vectors are processed!\n");
     }
 }
 

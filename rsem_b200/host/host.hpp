@@ -7,6 +7,7 @@
 // template classes, SoA read/hit stores instead of streams of objects.
 #pragma once
 
+#include <algorithm>
 #include <atomic>
 #include <cstdint>
 #include <cstdio>
@@ -338,6 +339,63 @@ rsem_b200_sim_params sim_params(const SimReference& ref, const SimSample& s, uin
 using SimNext = std::function<void(const char* text[2], uint64_t bytes[2], uint64_t* n)>;
 uint64_t write_sim_reads(const SimNext& next, FILE* const* os, int n_os, const Say* gen, double& t_next, double& t_write);
 
+// ---- ci_stages.cpp: the per-sample stages of rsem-calculate-credibility-intervals, which
+// rsem-calculate-credibility-intervals-batch runs for each manifest line --------------------------------------------------
+struct CiReference {   // refName.seq (lengths), refName.grp and, for an allele-specific reference, .gt / .ta
+    std::string name;
+    RefData refs;
+    std::vector<int> gi, gt, ta;
+    bool alleleS = false;
+    int m() const { return (int)gi.size() - 1; }
+    int m_trans() const { return alleleS ? (int)ta.size() - 1 : 0; }
+};
+void load_ci_reference(const std::string& refName, CiReference& ref);
+// the arguments after reference_name (calcCI.cpp:520-540)
+struct CiArgs {
+    std::string imdName, statName;
+    double confidence = 0, pseudoC = 1.0;
+    int nCV = 0, nSpC = 0, nMB = 0, nThreads = 1;
+    bool hasSeed = false, quiet = false;
+    uint32_t seed = 0;
+    int64_t n_samples() const { return (int64_t)nCV * nSpC; }
+    int samplers() const { return std::min(nThreads, nCV); }   // one per count-vector file (calcCI.cpp:172)
+};
+// imdName statName confidence nCV nSpC nMB [-p #Threads] [--seed seed] [--pseudo-count c] [-q] (f.size() >= 6); returns
+// "" or why -p is refused.  whole_seed: refuse a --seed without a value or with anything but digits (the batch); else the
+// seed is read digit by digit whatever it holds, as the reference does
+std::string parse_ci_args(const std::vector<std::string>& f, CiArgs& a, bool whole_seed);
+std::string ci_sample_count_error(const CiArgs& a, int M);   // nCV, nSpC positive, nCV * nSpC below 2^31; "" or why
+std::string ci_memory_error(const CiArgs& a, int M);         // nMB holds one sample row (Buffer.h:18-20); "" or why
+// statName.model -> the expected effective lengths and mw (dies as the reference does on a file it cannot read)
+void load_ci_model(const CiReference& ref, const CiArgs& a, std::vector<double>& eel, std::vector<double>& mw);
+// imdName.countvectors<t> for t < samplers(), one parser thread per file; dies when a file is missing or cannot be
+// parsed, or when the files do not hold nCV vectors (with isolate, die() throws on the parser threads and the first
+// failure is raised on the calling thread).  first[t]: the index of file t's first sample.
+struct CiSample {
+    std::vector<double> eel, mw;
+    std::vector<std::vector<int32_t>> cvs;
+    std::vector<int64_t> first;
+};
+void load_ci_vectors(const CiArgs& a, int M, CiSample& s, bool isolate);
+// the gene ranges of the reference's Phase II threads (calcCI.cpp:402-420), from the line's -p
+std::vector<int32_t> ci_parts(int nThreads, int M, const std::vector<int>& gi);
+// the run's parameters; the pointers are into ref and parts
+rsem_b200_ci_params ci_params(const CiReference& ref, const CiArgs& a, const std::vector<int32_t>& parts, uint64_t budget);
+// Phase I after ci_begin: one sampler thread per file pushes its rows as it draws them; the count vectors are released
+// as each thread ends.  progress (may be null) gets the samplers' lines from their threads.  With isolate, die() throws
+// on the sampler threads and the first failure is raised on the calling thread.  Returns the samplers' summed seconds.
+double ci_sample_rows(rsem_b200_ctx* ctx, const CiArgs& a, int M, CiSample& s, uint32_t seed, const Say* progress, bool isolate);
+// ci_end: the intervals of every transcript, gene and isoform, 6 floats each
+struct CiIntervals {
+    std::vector<float> tr, gene, iso;
+    rsem_b200_ci_stats st{};
+};
+void ci_intervals(rsem_b200_ctx* ctx, const CiReference& ref, CiIntervals& out);
+// the Phase II threads' progress lines (calcCI.cpp:360), the rows appended to imdName.iso_res / .gene_res (and
+// .allele_res) and "All credibility intervals are calculated!"; `say` (may be null) gets the lines
+void write_ci_sample(const CiReference& ref, const CiArgs& a, const std::vector<int32_t>& parts, const CiIntervals& r,
+                     const Say* say);
+
 // ---- alignment files for -b: SAM / BAM in, BAM out (bam.cpp; BamWriter.h, sam_utils.h, SamHeader.cpp) -----------------
 struct BamRecord {
     std::vector<uint8_t> data;  // the record as BAM stores it, without the leading block_size
@@ -490,14 +548,16 @@ struct DieThrows {
 };
 // One context per entry of `devices`, created on host threads.  arena[k] is lane k's batch arena: RSEM_B200_BATCH_ARENA_BYTES
 // when it is set and not 0; else, with one entry, 0 (the batch's own default); else half of the device memory free before the first
-// context on the lane's device, divided by the entries naming that device.  err: the first device that could not be
-// opened, once every creation has returned (the caller ends the run).
+// context on the lane's device, divided by the entries naming that device.  free[k]: from open_lanes_measured, the
+// device memory free on lane k's device before its first context (from open_lanes, 0 unless arena needed it).  err: the
+// first device that could not be opened, once every creation has returned (the caller ends the run).
 struct LaneContexts {
     std::vector<rsem_b200_ctx*> ctx;
-    std::vector<uint64_t> arena;
+    std::vector<uint64_t> arena, free;
     std::string err;
 };
 LaneContexts open_lanes(const std::vector<int>& devices);
+LaneContexts open_lanes_measured(const std::vector<int>& devices);
 // The manifest lines, handed to the lanes in manifest order; the first failure stops the handing out.
 class Claims {
   public:

@@ -24,11 +24,13 @@ std::vector<int> gpu_devices() {
     return devices;
 }
 
-LaneContexts open_lanes(const std::vector<int>& devices) {
+namespace {
+
+LaneContexts open_contexts(const std::vector<int>& devices, bool want_free) {
     const size_t n = devices.size();
     LaneContexts out;
     out.ctx.assign(n, nullptr);
-    out.arena.assign(n, 0);
+    out.free.assign(n, 0);
     const char* e = getenv("RSEM_B200_BATCH_ARENA_BYTES");
     const uint64_t set = e ? strtoull(e, nullptr, 10) : 0;   // 0 is the default, as unset
     out.arena.assign(n, set);
@@ -43,13 +45,16 @@ LaneContexts open_lanes(const std::vector<int>& devices) {
         for (size_t k = 0; k < n; ++k)
             if (devices[k] == d) mine.push_back(k);
         const std::string where = n > 1 ? "device " + std::to_string(d) + ": " : "";
-        if (share) {
+        if (share || want_free) {
             uint64_t free_b = 0;
             if (rsem_b200_device_free_bytes(d, &free_b) != 0) {
                 err[mine[0]] = "rsem_b200: " + where + "device_free_bytes failed: " + rsem_b200_last_error();
                 return;
             }
-            for (size_t k : mine) out.arena[k] = free_b / 2 / mine.size();
+            for (size_t k : mine) {
+                out.free[k] = free_b;
+                if (share) out.arena[k] = free_b / 2 / mine.size();
+            }
         }
         for (size_t k : mine)
             if (rsem_b200_ctx_create(d, &out.ctx[k]) != 0) {
@@ -70,6 +75,12 @@ LaneContexts open_lanes(const std::vector<int>& devices) {
         }
     return out;
 }
+
+}  // namespace
+
+LaneContexts open_lanes(const std::vector<int>& devices) { return open_contexts(devices, false); }
+
+LaneContexts open_lanes_measured(const std::vector<int>& devices) { return open_contexts(devices, true); }
 
 size_t Claims::next() {
     if (failed_) return n_;
